@@ -50,14 +50,10 @@ class B200zkError(RuntimeError):
         self.code = code
 
 
-def _load():
-    if not os.path.exists(LIB_PATH):
-        raise ImportError(
-            f"{LIB_PATH} not built; run `python scroll-prover_b200/build.py` (needs nvcc). There is no CPU fallback."
-        )
-    lib = C.CDLL(LIB_PATH)
+def _signatures():
+    """argtypes of every int32_t-returning symbol of include/b200zk.h."""
     vp, u64, u32, i32 = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int32
-    sig = {
+    return {
         "b200zk_ctx_create": [C.POINTER(C.c_int), C.c_int, C.POINTER(vp)],
         "b200zk_ctx_destroy": [vp],
         "b200zk_ctx_set_stream": [vp, vp],
@@ -119,25 +115,25 @@ def _load():
         "b200zk_msm_last_stats": [vp, C.POINTER(u32), C.POINTER(u32), C.POINTER(u64)],
         "b200zk_msm_total_adds": [vp, C.POINTER(u64), C.c_int],
     }
-    for name, args in sig.items():
+
+
+_SIGNATURES = _signatures()
+ABI_SYMBOLS = [*_SIGNATURES, "b200zk_last_error"]
+
+
+def _load():
+    if not os.path.exists(LIB_PATH):
+        raise ImportError(
+            f"{LIB_PATH} not built; run `python scroll-prover_b200/build.py` (needs nvcc). There is no CPU fallback."
+        )
+    lib = C.CDLL(LIB_PATH)
+    for name, args in _SIGNATURES.items():
         fn = getattr(lib, name)
         fn.argtypes = args
-        fn.restype = i32
-    lib.b200zk_last_error.argtypes = [vp]
+        fn.restype = C.c_int32
+    lib.b200zk_last_error.argtypes = [C.c_void_p]
     lib.b200zk_last_error.restype = C.c_char_p
     return lib
-
-
-ABI_SYMBOLS = [
-    "b200zk_ctx_create", "b200zk_ctx_destroy", "b200zk_last_error", "b200zk_ctx_set_stream", "b200zk_ctx_synchronize",
-    "b200zk_ctx_launch_count", "b200zk_buf_alloc", "b200zk_buf_free", "b200zk_buf_upload", "b200zk_buf_download",
-    "b200zk_srs_register", "b200zk_srs_set_precompute", "b200zk_srs_release", "b200zk_srs_len", "b200zk_msm_g1", "b200zk_msm_g1_bases", "b200zk_msm_g1_batch", "b200zk_msm_g1_range", "b200zk_msm_g1_sharded",
-    "b200zk_comm_unique_id", "b200zk_ctx_comm_init", "b200zk_ctx_comm_info", "b200zk_shard_range", "b200zk_g1_sum",
-    "b200zk_g1_generator_mul_batch", "b200zk_fft_g1", "b200zk_g_to_lagrange", "b200zk_ntt_fr", "b200zk_ntt_fr_ext", "b200zk_ctx_set_overlap", "b200zk_run_column_jobs", "b200zk_commit_columns", "b200zk_poly_add", "b200zk_poly_sub",
-    "b200zk_poly_mul", "b200zk_poly_scale", "b200zk_poly_axpy", "b200zk_eval_poly", "b200zk_inner_product", "b200zk_batch_invert",
-    "b200zk_kate_division", "b200zk_prefix_scan", "b200zk_poly_lincomb", "b200zk_permutation_product", "b200zk_logup_running_sum", "b200zk_graph_create", "b200zk_graph_check",
-    "b200zk_graph_destroy", "b200zk_graph_info", "b200zk_graph_evaluate", "b200zk_graph_evaluate_rows", "b200zk_allgather_rows", "b200zk_debug_field_op", "b200zk_profile_enable", "b200zk_profile_reset", "b200zk_profile_read", "b200zk_msm_set_window", "b200zk_msm_last_stats", "b200zk_msm_total_adds",
-]
 
 _lib = None
 
@@ -163,6 +159,13 @@ def _ptr(x):
         return C.c_void_p(x.data_ptr()), x
     a = np.ascontiguousarray(x)
     return C.c_void_p(a.ctypes.data), a
+
+
+def _write_back(x, keep):
+    """After an in-place call: copy the result into x when _ptr had to hand the library a contiguous copy of it."""
+    if not _is_torch(x) and keep is not x:
+        x[...] = keep.reshape(np.asarray(x).shape)
+    return x
 
 
 def fr_from_int(v: int) -> np.ndarray:
@@ -341,9 +344,7 @@ class Context:
         pa, k1 = _ptr(jac_points)
         po, k2 = _ptr(omega)
         self._ck(lib().b200zk_fft_g1(self._h, pa, log_n, po))
-        if not _is_torch(jac_points) and k1 is not jac_points:
-            jac_points[...] = k1.reshape(np.asarray(jac_points).shape)
-        return jac_points
+        return _write_back(jac_points, k1)
 
     def g_to_lagrange(self, g, k: int, out=None):
         """poly::kzg::commitment::g_to_lagrange (Params::downsize): affine (2^k, 8) -> affine (2^k, 8)."""
@@ -362,9 +363,7 @@ class Context:
         pa, k1 = _ptr(a)
         po, k2 = _ptr(omega)
         self._ck(lib().b200zk_ntt_fr(self._h, pa, log_n, po, int(inverse_scale), coset_mode))
-        if not _is_torch(a) and k1 is not a:
-            a[...] = k1.reshape(np.asarray(a).shape)
-        return a
+        return _write_back(a, k1)
 
     def ntt_ext(self, a_in, log_in: int, out, log_n: int, omega, inverse_scale: bool = False, coset_mode: int = COSET_NONE):
         assert _count(a_in, 32) == 1 << log_in and _count(out, 32) == 1 << log_n
@@ -426,35 +425,27 @@ class Context:
         return Graph(self, calcs, constants, rotations)
 
     # ---- poly ops
-    def _ew(self, fn, r, *args, n):
-        ptrs = [_ptr(x) for x in (r,) + args]
-        self._ck(fn(self._h, *[p for p, _ in ptrs], n))
-        return r
+    def _ew(self, fn, a, *args, out=None):
+        """fn(ctx, out, a, *args, n) over the n = len(a) elements of a; out is allocated like a when not given."""
+        out = _like(a) if out is None else out
+        ptrs = [_ptr(x) for x in (out, a) + args]
+        self._ck(fn(self._h, *[p for p, _ in ptrs], _count(a, 32)))
+        return out
 
     def poly_add(self, a, b, out=None):
-        n = _count(a, 32)
-        out = _like(a) if out is None else out
-        return self._ew(lib().b200zk_poly_add, out, a, b, n=n)
+        return self._ew(lib().b200zk_poly_add, a, b, out=out)
 
     def poly_sub(self, a, b, out=None):
-        n = _count(a, 32)
-        out = _like(a) if out is None else out
-        return self._ew(lib().b200zk_poly_sub, out, a, b, n=n)
+        return self._ew(lib().b200zk_poly_sub, a, b, out=out)
 
     def poly_mul(self, a, b, out=None):
-        n = _count(a, 32)
-        out = _like(a) if out is None else out
-        return self._ew(lib().b200zk_poly_mul, out, a, b, n=n)
+        return self._ew(lib().b200zk_poly_mul, a, b, out=out)
 
     def poly_scale(self, a, s, out=None):
-        n = _count(a, 32)
-        out = _like(a) if out is None else out
-        return self._ew(lib().b200zk_poly_scale, out, a, s, n=n)
+        return self._ew(lib().b200zk_poly_scale, a, s, out=out)
 
     def poly_axpy(self, a, s, b, out=None):
-        n = _count(a, 32)
-        out = _like(a) if out is None else out
-        return self._ew(lib().b200zk_poly_axpy, out, a, s, b, n=n)
+        return self._ew(lib().b200zk_poly_axpy, a, s, b, out=out)
 
     def eval_polynomial(self, poly, point) -> np.ndarray:
         n = _count(poly, 32)
@@ -477,9 +468,7 @@ class Context:
         n = _count(data, 32)
         p, k = _ptr(data)
         self._ck(lib().b200zk_batch_invert(self._h, p, n))
-        if not _is_torch(data) and k is not data:
-            data[...] = k.reshape(np.asarray(data).shape)
-        return data
+        return _write_back(data, k)
 
     def kate_division(self, a, b) -> np.ndarray:
         n = _count(a, 32)
@@ -612,19 +601,10 @@ class Graph:
     def __init__(self, ctx: Context, calcs, constants, rotations):
         self.ctx = ctx
         self._h = C.c_void_p()
-        parts = []
-        arr = (_Calculation * max(1, len(calcs)))()
-        for i, (op, a, b, ps) in enumerate(calcs):
-            arr[i].op = op
-            arr[i].a = _ValueSource(*a)
-            arr[i].b = _ValueSource(*(b if b is not None else (0, 0, 0)))
-            arr[i].parts_offset = len(parts)
-            arr[i].parts_len = len(ps or [])
-            parts.extend(ps or [])
-        parr = (_ValueSource * max(1, len(parts)))(*[_ValueSource(*q) for q in parts])
+        arr, parr, n_parts = _pack_calcs(calcs)
         consts = np.ascontiguousarray(np.asarray(constants, dtype=np.uint64).reshape(-1, 4))
         rots = np.ascontiguousarray(np.asarray(rotations, dtype=np.int32).reshape(-1))
-        ctx._ck(lib().b200zk_graph_create(ctx._h, C.cast(arr, C.c_void_p), len(calcs), C.cast(parr, C.c_void_p), len(parts),
+        ctx._ck(lib().b200zk_graph_create(ctx._h, C.cast(arr, C.c_void_p), len(calcs), C.cast(parr, C.c_void_p), n_parts,
                                           C.c_void_p(consts.ctypes.data), len(consts), C.c_void_p(rots.ctypes.data), len(rots),
                                           C.byref(self._h)))
 
@@ -638,19 +618,6 @@ class Graph:
         """values[row] = GraphEvaluator::evaluate(.., previous_value = values[row], ..) for every row of the extended domain
         (rows = (first, count): only that slice -- evaluate_h sharded by row range, see Context.allgather_rows)."""
         assert _count(values, 32) == 1 << log_size
-        if rows is not None:
-            zero = np.zeros(4, np.uint64)
-            tf, kf = Context._dev_table(fixed)
-            ta, ka = Context._dev_table(advice)
-            ti, ki = Context._dev_table(instance)
-            ch = np.ascontiguousarray(np.asarray(challenges if challenges is not None else [], dtype=np.uint64).reshape(-1, 4))
-            sc = [_ptr(zero if v is None else v) for v in (beta, gamma, theta, y)]
-            pw, kw = _ptr(extended_omega)
-            pv, kv = _ptr(values)
-            self.ctx._ck(lib().b200zk_graph_evaluate_rows(self.ctx._h, self._h, tf, len(fixed), ta, len(advice), ti, len(instance),
-                                                          C.c_void_p(ch.ctypes.data) if len(ch) else None, len(ch), *[p for p, _ in sc], pw,
-                                                          pv, log_size, rot_scale, rows[0], rows[1]))
-            return values
         zero = np.zeros(4, np.uint64)
         tf, kf = Context._dev_table(fixed)
         ta, ka = Context._dev_table(advice)
@@ -659,9 +626,12 @@ class Graph:
         sc = [_ptr(zero if v is None else v) for v in (beta, gamma, theta, y)]
         pw, kw = _ptr(extended_omega)
         pv, kv = _ptr(values)
-        self.ctx._ck(lib().b200zk_graph_evaluate(self.ctx._h, self._h, tf, len(fixed), ta, len(advice), ti, len(instance),
-                                                 C.c_void_p(ch.ctypes.data) if len(ch) else None, len(ch), *[p for p, _ in sc], pw, pv,
-                                                 log_size, rot_scale))
+        args = (self.ctx._h, self._h, tf, len(fixed), ta, len(advice), ti, len(instance), C.c_void_p(ch.ctypes.data) if len(ch) else None,
+                len(ch), *[p for p, _ in sc], pw, pv, log_size, rot_scale)
+        if rows is None:
+            self.ctx._ck(lib().b200zk_graph_evaluate(*args))
+        else:
+            self.ctx._ck(lib().b200zk_graph_evaluate_rows(*args, rows[0], rows[1]))
         return values
 
     def release(self):

@@ -8,14 +8,6 @@
 #include "ec.cuh"
 
 namespace b200zk {
-int32_t msm_run(b200zk_ctx* ctx, const Affine* bases, const Fr* scalars, uint64_t n, Jacobian* out_dev, uint32_t pre_c,
-                uint64_t pre_stride);
-int32_t msm_run_batch(b200zk_ctx* ctx, const Affine* bases, const Fr* const* cols, uint32_t batch, uint64_t n, Jacobian* out_dev,
-                      uint32_t pre_c, uint64_t pre_stride);
-uint32_t msm_max_batch(uint64_t n, uint32_t pre_c);
-uint32_t msm_pick_window_precomputed(uint64_t n);
-int32_t srs_precompute_run(b200zk_ctx* ctx, Affine* tables, uint64_t n, uint32_t c, uint32_t W);
-int32_t g1_sum_run(b200zk_ctx* ctx, const Jacobian* pts, uint64_t count, Jacobian* out_dev);
 int32_t g1_generator_mul_run(b200zk_ctx* ctx, const Fr* scalars, uint64_t n, Affine* out);
 int32_t poly_ew(b200zk_ctx* ctx, int op, Fr* r, const Fr* a, const Fr* b, const Fr& s, uint64_t n);
 int32_t eval_poly(b200zk_ctx* ctx, const Fr* poly, uint64_t n, const Fr& x, Fr* out_dev);
@@ -170,43 +162,10 @@ int32_t b200zk_srs_register(b200zk_ctx* ctx, const void* g1_affine, uint64_t n, 
     s->ctx = ctx;
     s->n = n;
     s->tag = tag;
-    s->dev_bases = nullptr;
-    s->pre_c = 0;
-    s->pre_W = 1;
-    size_t bytes = sizeof(Affine) * (n ? n : 1);
-    if (ctx->srs_precompute && n >= (1ull << 16)) {
-        // keep 2^(c*w) * P_i for every window w: all windows then share ONE bucket set (no per-window reduction, no
-        // Horner doublings) and a wider window pays off.  Costs W x the base storage; skipped when memory is short.
-        uint32_t c = msm_pick_window_precomputed(n), W = 254 / c + 1;
-        size_t free_b = 0, total_b = 0;
-        if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && (double)bytes * W < 0.35 * (double)free_b) {
-            s->pre_c = c;
-            s->pre_W = W;
-            bytes *= W;
-        }
-    }
-    cudaError_t e = cudaMalloc(&s->dev_bases, bytes);
-    if (e != cudaSuccess) {
-        (void)cudaGetLastError();
+    int32_t rc = srs_init(ctx, s, g1_affine);
+    if (rc != B200ZK_OK) {
         delete s;
-        return fail(ctx, B200ZK_E_OOM, "srs_register: cudaMalloc(%zu) failed", bytes);
-    }
-    cudaMemcpyKind kind = is_device_ptr(g1_affine) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    e = n ? cudaMemcpyAsync(s->dev_bases, g1_affine, sizeof(Affine) * n, kind, ctx->stream) : cudaSuccess;
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) {
-        cudaFree(s->dev_bases);
-        delete s;
-        return fail(ctx, B200ZK_E_CUDA, "srs_register: upload failed: %s", cudaGetErrorString(e));
-    }
-    if (s->pre_c) {
-        int32_t rc = srs_precompute_run(ctx, (Affine*)s->dev_bases, n, s->pre_c, s->pre_W);
-        if (rc == B200ZK_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = B200ZK_E_CUDA;
-        if (rc != B200ZK_OK) {
-            cudaFree(s->dev_bases);
-            delete s;
-            return fail(ctx, rc, "srs_register: precomputation failed");
-        }
+        return rc;
     }
     *out = s;
     return B200ZK_OK;
@@ -216,7 +175,7 @@ int32_t b200zk_srs_release(b200zk_ctx* ctx, b200zk_srs* srs) {
     if (!srs) return B200ZK_OK;
     Guard g(ctx);
     B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (srs->dev_bases) cudaFree(srs->dev_bases);
+    srs_free(srs);
     delete srs;
     return B200ZK_OK;
 }
@@ -227,16 +186,6 @@ int32_t b200zk_srs_len(const b200zk_srs* srs, uint64_t* out) {
 }
 
 // ---- MSM ---------------------------------------------------------------------------------------
-static int32_t msm_common(b200zk_ctx* ctx, const Affine* bases_dev, const void* scalars, uint64_t n, void* out96,
-                          uint32_t pre_c = 0, uint64_t pre_stride = 0) {
-    const void* sc_dev = nullptr;
-    if (n) B2_TRY(stage_in(ctx, ctx->stage_in, scalars, sizeof(Fr) * n, &sc_dev));
-    B2_TRY(scratch_reserve(ctx, ctx->stage_out, 256));
-    Jacobian* res = (Jacobian*)ctx->stage_out.p;
-    B2_TRY(msm_run(ctx, bases_dev, (const Fr*)sc_dev, n, res, pre_c, pre_stride));
-    return deliver(ctx, out96, res, sizeof(Jacobian));
-}
-
 int32_t b200zk_msm_g1(b200zk_ctx* ctx, const b200zk_srs* srs, const void* scalars, uint64_t n, void* out_jacobian96) {
     CHECK_CTX(ctx);
     if (!srs || !out_jacobian96 || (n && !scalars)) return fail(ctx, B200ZK_E_INVALID, "msm_g1: null pointer");
@@ -245,10 +194,11 @@ int32_t b200zk_msm_g1(b200zk_ctx* ctx, const b200zk_srs* srs, const void* scalar
         return fail(ctx, B200ZK_E_INVALID, "msm_g1: %llu scalars but only %llu bases (assert_eq!(coeffs.len(), bases.len()))",
                     (unsigned long long)n, (unsigned long long)srs->n);
     Guard g(ctx);
-    // a commit over a short prefix of a large precomputed SRS is cheaper with the plain bases (table 0) and a window
-    // sized for n than with the handle's wide window (2^(c-1) buckets to reduce)
-    uint32_t pre_c = (srs->pre_c && n * 16 >= srs->n) ? srs->pre_c : 0;
-    return msm_common(ctx, (const Affine*)srs->dev_bases, scalars, n, out_jacobian96, pre_c, srs->n);
+    const void* sc_dev = nullptr;
+    if (n) B2_TRY(stage_in(ctx, ctx->stage_in, scalars, sizeof(Fr) * n, &sc_dev));
+    const Fr* sc = (const Fr*)sc_dev;
+    return out_small(ctx, out_jacobian96, sizeof(Jacobian),
+                     [&](void* res) { return msm_srs(ctx, srs, 0, &sc, 1, n, (Jacobian*)res); });
 }
 
 int32_t b200zk_msm_g1_batch(b200zk_ctx* ctx, const b200zk_srs* srs, const void* const* scalars, uint32_t count, uint64_t n,
@@ -264,8 +214,7 @@ int32_t b200zk_msm_g1_batch(b200zk_ctx* ctx, const b200zk_srs* srs, const void* 
     Guard g(ctx);
     if (!count) return B200ZK_OK;
     try {
-    const uint32_t pre_c = (srs->pre_c && n * 16 >= srs->n) ? srs->pre_c : 0;
-    const uint32_t bmax = msm_max_batch(n, pre_c);
+    const uint32_t bmax = msm_srs_max_batch(srs, n);
     B2_TRY(scratch_reserve(ctx, ctx->stage_out, sizeof(Jacobian) * count));
     Jacobian* res = (Jacobian*)ctx->stage_out.p;
     size_t host_bytes = 0;  // staging for the host-resident columns of one batch
@@ -289,7 +238,7 @@ int32_t b200zk_msm_g1_batch(b200zk_ctx* ctx, const b200zk_srs* srs, const void* 
             }
             cols[q] = (const Fr*)p;
         }
-        B2_TRY(msm_run_batch(ctx, (const Affine*)srs->dev_bases, cols.data(), len, n, res + j0, pre_c, srs->n));
+        B2_TRY(msm_srs(ctx, srs, 0, cols.data(), len, n, res + j0));
         // the staging buffer is reused by the next batch, and the caller's host columns must not be read after we return
         if (host_bytes && (j0 + bmax < count || is_device_ptr(out_jacobian96))) B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
@@ -303,10 +252,11 @@ int32_t b200zk_msm_g1_bases(b200zk_ctx* ctx, const void* g1_affine, const void* 
     CHECK_CTX(ctx);
     if (!out_jacobian96 || (n && (!scalars || !g1_affine))) return fail(ctx, B200ZK_E_INVALID, "msm_g1_bases: null pointer");
     Guard g(ctx);
-    const void* b_dev = nullptr;
-    if (n) B2_TRY(stage_in(ctx, ctx->misc, g1_affine, sizeof(Affine) * n, &b_dev));
-    // NB: ctx->misc is not used by msm_run
-    return msm_common(ctx, (const Affine*)b_dev, scalars, n, out_jacobian96);
+    const void *b_dev = nullptr, *sc_dev = nullptr;
+    if (n) B2_TRY(stage_in(ctx, ctx->misc, g1_affine, sizeof(Affine) * n, &b_dev));  // NB: ctx->misc is not used by the MSM
+    if (n) B2_TRY(stage_in(ctx, ctx->stage_in, scalars, sizeof(Fr) * n, &sc_dev));
+    return out_small(ctx, out_jacobian96, sizeof(Jacobian),
+                     [&](void* res) { return msm_bases(ctx, (const Affine*)b_dev, (const Fr*)sc_dev, n, (Jacobian*)res); });
 }
 
 int32_t b200zk_g1_sum(b200zk_ctx* ctx, const void* jacobian_points, uint64_t count, void* out_jacobian96) {
@@ -315,10 +265,8 @@ int32_t b200zk_g1_sum(b200zk_ctx* ctx, const void* jacobian_points, uint64_t cou
     Guard g(ctx);
     const void* p_dev = nullptr;
     if (count) B2_TRY(stage_in(ctx, ctx->stage_in, jacobian_points, sizeof(Jacobian) * count, &p_dev));
-    B2_TRY(scratch_reserve(ctx, ctx->stage_out, 256));
-    Jacobian* res = (Jacobian*)ctx->stage_out.p;
-    B2_TRY(g1_sum_run(ctx, (const Jacobian*)p_dev, count, res));
-    return deliver(ctx, out_jacobian96, res, sizeof(Jacobian));
+    return out_small(ctx, out_jacobian96, sizeof(Jacobian),
+                     [&](void* res) { return g1_sum_run(ctx, (const Jacobian*)p_dev, count, (Jacobian*)res); });
 }
 
 int32_t b200zk_g1_generator_mul_batch(b200zk_ctx* ctx, const void* scalars, uint64_t n, void* out_affine) {
@@ -328,15 +276,10 @@ int32_t b200zk_g1_generator_mul_batch(b200zk_ctx* ctx, const void* scalars, uint
     if (!n) return B200ZK_OK;
     const void* sc_dev = nullptr;
     B2_TRY(stage_in(ctx, ctx->stage_in, scalars, sizeof(Fr) * n, &sc_dev));
-    bool out_dev = is_device_ptr(out_affine);
-    Affine* res = (Affine*)out_affine;
-    if (!out_dev) {
-        B2_TRY(scratch_reserve(ctx, ctx->stage_out, sizeof(Affine) * n));
-        res = (Affine*)ctx->stage_out.p;
-    }
-    B2_TRY(g1_generator_mul_run(ctx, (const Fr*)sc_dev, n, res));
-    if (!out_dev) return d2h(ctx, out_affine, res, sizeof(Affine) * n);
-    return B200ZK_OK;
+    void* res = nullptr;
+    B2_TRY(out_begin(ctx, out_affine, sizeof(Affine) * n, &res));
+    B2_TRY(g1_generator_mul_run(ctx, (const Fr*)sc_dev, n, (Affine*)res));
+    return out_end(ctx, out_affine, res, sizeof(Affine) * n);
 }
 
 // ---- FFT over G1 (SRS tooling) -------------------------------------------------------------------
@@ -346,15 +289,10 @@ static int32_t g1_fft_common(b200zk_ctx* ctx, const void* in, bool from_jac, voi
     size_t in_bytes = (from_jac ? sizeof(Jacobian) : sizeof(Affine)) * n, out_bytes = (to_jac ? sizeof(Jacobian) : sizeof(Affine)) * n;
     const void* in_dev = nullptr;
     B2_TRY(stage_in(ctx, ctx->stage_in, in, in_bytes, &in_dev));
-    bool out_is_dev = is_device_ptr(out);
-    void* out_dev = out;
-    if (!out_is_dev) {
-        B2_TRY(scratch_reserve(ctx, ctx->stage_out, out_bytes));
-        out_dev = ctx->stage_out.p;
-    }
+    void* out_dev = nullptr;
+    B2_TRY(out_begin(ctx, out, out_bytes, &out_dev));
     B2_TRY(g1_fft_run(ctx, in_dev, from_jac, out_dev, to_jac, log_n, omega, scale));
-    if (!out_is_dev) return d2h(ctx, out, out_dev, out_bytes);
-    return B200ZK_OK;
+    return out_end(ctx, out, out_dev, out_bytes);
 }
 
 int32_t b200zk_fft_g1(b200zk_ctx* ctx, void* jacobian_points, uint32_t log_n, const void* omega32) {
@@ -393,23 +331,18 @@ int32_t b200zk_ntt_fr_ext(b200zk_ctx* ctx, const void* in, uint32_t log_in, void
     Fr omega;
     B2_TRY(read_fr(ctx, omega32, &omega));
     size_t in_bytes = sizeof(Fr) << log_in, out_bytes = sizeof(Fr) << log_n;
-    bool out_is_dev = is_device_ptr(out);
-    Fr* out_dev = (Fr*)out;
-    if (!out_is_dev) {
-        B2_TRY(scratch_reserve(ctx, ctx->stage_out, out_bytes));
-        out_dev = (Fr*)ctx->stage_out.p;
-    }
+    void* out_dev = nullptr;
+    B2_TRY(out_begin(ctx, out, out_bytes, &out_dev));
     const void* in_dev = nullptr;
-    if (!is_device_ptr(in) && !out_is_dev && log_in == log_n) {
+    if (!is_device_ptr(in) && out_dev != out && log_in == log_n) {
         // host in / host out of equal size: upload straight into the output staging buffer and run in place
         B2_TRY(h2d(ctx, out_dev, in, in_bytes));
         in_dev = out_dev;
     } else {
         B2_TRY(stage_in(ctx, ctx->stage_in, in, in_bytes, &in_dev));
     }
-    B2_TRY(ntt_run(ctx, (const Fr*)in_dev, log_in, out_dev, log_n, omega, inverse_scale, coset_mode));
-    if (!out_is_dev) return d2h(ctx, out, out_dev, out_bytes);
-    return B200ZK_OK;
+    B2_TRY(ntt_run(ctx, (const Fr*)in_dev, log_in, (Fr*)out_dev, log_n, omega, inverse_scale, coset_mode));
+    return out_end(ctx, out, out_dev, out_bytes);
 }
 
 int32_t b200zk_ntt_fr(b200zk_ctx* ctx, void* data, uint32_t log_n, const void* omega32, int inverse_scale, int coset_mode) {
@@ -434,7 +367,7 @@ static int32_t pipeline_init(b200zk_ctx* ctx) {
 // One call = a list of independent per-column jobs of plonk::create_proof whose inputs are in HOST memory (pinned for
 // overlap) or already on the device.  Jobs are taken in GROUPS: a group is uploaded (copy stream) while the previous one
 // computes, and the commitments of a group's consecutive jobs over the same SRS go through ONE batched MSM pipeline
-// (msm_run_batch) -- for 2^20-row columns that is up to 16 columns per pipeline, a 2^24+ column is a group of its own.
+// (msm_srs) -- for 2^20-row columns that is up to 16 columns per pipeline, a 2^24+ column is a group of its own.
 // No host synchronisation inside the loop.
 static int32_t run_column_jobs_impl(b200zk_ctx* ctx, const b200zk_column_job* jobs, uint32_t count, uint32_t k, const void* omega_inv32,
                                     const void* extended_omega32, const void* extended_omega_inv32, uint32_t extended_k,
@@ -483,11 +416,10 @@ static int32_t run_column_jobs_impl(b200zk_ctx* ctx, const b200zk_column_job* jo
     const size_t col_bytes = sizeof(Fr) * n, ext_bytes = sizeof(Fr) << extended_k;
 
     // ---- groups: [first, first + len); a mode-4 job (2^extended_k input values) is always a group of its own
-    auto pre_of = [&](const b200zk_srs* s) -> uint32_t { return (n * 16 >= s->n) ? s->pre_c : 0; };
     uint32_t gmax = 1;
     for (uint32_t j = 0; j < count; ++j)
         if (jobs[j].mode <= 2) {
-            gmax = msm_max_batch(n, pre_of(jobs[j].srs));
+            gmax = msm_srs_max_batch(jobs[j].srs, n);
             break;
         }
     if (gmax > 16) gmax = 16;
@@ -526,23 +458,18 @@ static int32_t run_column_jobs_impl(b200zk_ctx* ctx, const b200zk_column_job* jo
     // are latency- or memory-bound and overlap with the other stream's butterflies.
     const bool overlap = ctx->overlap && (any_coeff || any_quot || any_ext) && any_commit;
     cudaStream_t main_stream = ctx->stream, ntt_stream = overlap ? ctx->aux_stream : ctx->stream;
-    struct StreamSwap {  // ntt_run / msm_run launch on ctx->stream
+    struct StreamSwap {  // ntt_run / msm_srs launch on ctx->stream
         b200zk_ctx* c;
         cudaStream_t saved;
         StreamSwap(b200zk_ctx* c_, cudaStream_t s) : c(c_), saved(c_->stream) { c->stream = s; }
         ~StreamSwap() { c->stream = saved; }
     };
-    if (any_coeff) {  // twiddle tables are built once, on the context stream, before the streams fork
+    // twiddle tables are built once, on the context stream, before the streams fork
+    const struct { bool used; Fr omega; uint32_t log_n; } twiddles[] = {
+        {any_coeff, omega_inv, k}, {any_ext && extended_k >= 1, ext_omega, extended_k}, {any_quot && extended_k >= 1, ext_omega_inv, extended_k}};
+    for (const auto& tw : twiddles) {
         const Fr* t = nullptr;
-        B2_TRY(ntt_get_table(ctx, omega_inv, k, &t));
-    }
-    if (any_ext && extended_k >= 1) {
-        const Fr* t = nullptr;
-        B2_TRY(ntt_get_table(ctx, ext_omega, extended_k, &t));
-    }
-    if (any_quot && extended_k >= 1) {
-        const Fr* t = nullptr;
-        B2_TRY(ntt_get_table(ctx, ext_omega_inv, extended_k, &t));
+        if (tw.used) B2_TRY(ntt_get_table(ctx, tw.omega, tw.log_n, &t));
     }
     // neither the copy stream nor the aux stream may overtake work already queued on the context stream
     B2_CUDA(ctx, cudaEventRecord(ctx->ev_fork, main_stream));
@@ -598,10 +525,9 @@ static int32_t run_column_jobs_impl(b200zk_ctx* ctx, const b200zk_column_job* jo
                     continue;
                 }
                 const b200zk_srs* srs = jobs[j].srs;
-                const uint32_t pre_c = pre_of(srs), bmax = msm_max_batch(n, pre_c);
                 uint32_t len = 1;
-                while (j + len < gr.first + gr.len && len < bmax && jobs[j + len].mode <= 2 && jobs[j + len].srs == srs) ++len;
-                B2_TRY(msm_run_batch(ctx, (const Affine*)srs->dev_bases, &src[j], len, n, commits + j, pre_c, srs->n));
+                while (j + len < gr.first + gr.len && jobs[j + len].mode <= 2 && jobs[j + len].srs == srs) ++len;
+                B2_TRY(msm_srs(ctx, srs, 0, &src[j], len, n, commits + j));
                 j += len;
             }
             if (host_in) {
@@ -684,15 +610,10 @@ static int32_t ew_common(b200zk_ctx* ctx, int op, void* r, const void* a, const 
     const void *a_dev = nullptr, *b_dev = nullptr;
     B2_TRY(stage_in(ctx, ctx->stage_in, a, bytes, &a_dev));
     if (need_b) B2_TRY(stage_in(ctx, ctx->ntt_work, b, bytes, &b_dev));
-    bool r_is_dev = is_device_ptr(r);
-    Fr* r_dev = (Fr*)r;
-    if (!r_is_dev) {
-        B2_TRY(scratch_reserve(ctx, ctx->stage_out, bytes));
-        r_dev = (Fr*)ctx->stage_out.p;
-    }
-    B2_TRY(poly_ew(ctx, op, r_dev, (const Fr*)a_dev, (const Fr*)b_dev, s, n));
-    if (!r_is_dev) return d2h(ctx, r, r_dev, bytes);
-    return B200ZK_OK;
+    void* r_dev = nullptr;
+    B2_TRY(out_begin(ctx, r, bytes, &r_dev));
+    B2_TRY(poly_ew(ctx, op, (Fr*)r_dev, (const Fr*)a_dev, (const Fr*)b_dev, s, n));
+    return out_end(ctx, r, r_dev, bytes);
 }
 int32_t b200zk_poly_add(b200zk_ctx* ctx, void* r, const void* a, const void* b, uint64_t n) { return ew_common(ctx, 0, r, a, b, nullptr, n); }
 int32_t b200zk_poly_sub(b200zk_ctx* ctx, void* r, const void* a, const void* b, uint64_t n) { return ew_common(ctx, 1, r, a, b, nullptr, n); }
@@ -708,33 +629,31 @@ int32_t b200zk_eval_poly(b200zk_ctx* ctx, const void* poly, uint64_t n, const vo
     Guard g(ctx);
     Fr x;
     B2_TRY(read_fr(ctx, point32, &x));
-    B2_TRY(scratch_reserve(ctx, ctx->stage_out, 256));
-    Fr* res = (Fr*)ctx->stage_out.p;
-    if (!n) {
-        B2_CUDA(ctx, cudaMemsetAsync(res, 0, sizeof(Fr), ctx->stream));
-    } else {
+    return out_small(ctx, out32, sizeof(Fr), [&](void* res) -> int32_t {
+        if (!n) {
+            B2_CUDA(ctx, cudaMemsetAsync(res, 0, sizeof(Fr), ctx->stream));
+            return B200ZK_OK;
+        }
         const void* p_dev = nullptr;
         B2_TRY(stage_in(ctx, ctx->stage_in, poly, sizeof(Fr) * n, &p_dev));
-        B2_TRY(eval_poly(ctx, (const Fr*)p_dev, n, x, res));
-    }
-    return deliver(ctx, out32, res, sizeof(Fr));
+        return eval_poly(ctx, (const Fr*)p_dev, n, x, (Fr*)res);
+    });
 }
 
 int32_t b200zk_inner_product(b200zk_ctx* ctx, const void* a, const void* b, uint64_t n, void* out32) {
     CHECK_CTX(ctx);
     if (!out32 || (n && (!a || !b))) return fail(ctx, B200ZK_E_INVALID, "inner_product: null pointer");
     Guard g(ctx);
-    B2_TRY(scratch_reserve(ctx, ctx->stage_out, 256));
-    Fr* res = (Fr*)ctx->stage_out.p;
-    if (!n) {
-        B2_CUDA(ctx, cudaMemsetAsync(res, 0, sizeof(Fr), ctx->stream));
-    } else {
+    return out_small(ctx, out32, sizeof(Fr), [&](void* res) -> int32_t {
+        if (!n) {
+            B2_CUDA(ctx, cudaMemsetAsync(res, 0, sizeof(Fr), ctx->stream));
+            return B200ZK_OK;
+        }
         const void *a_dev = nullptr, *b_dev = nullptr;
         B2_TRY(stage_in(ctx, ctx->stage_in, a, sizeof(Fr) * n, &a_dev));
         B2_TRY(stage_in(ctx, ctx->ntt_work, b, sizeof(Fr) * n, &b_dev));
-        B2_TRY(inner_product(ctx, (const Fr*)a_dev, (const Fr*)b_dev, n, res));
-    }
-    return deliver(ctx, out32, res, sizeof(Fr));
+        return inner_product(ctx, (const Fr*)a_dev, (const Fr*)b_dev, n, (Fr*)res);
+    });
 }
 
 int32_t b200zk_batch_invert(b200zk_ctx* ctx, void* data, uint64_t n) {
@@ -759,16 +678,11 @@ int32_t b200zk_kate_division(b200zk_ctx* ctx, void* q, const void* a, uint64_t n
     B2_TRY(read_fr(ctx, b32, &b));
     const void* a_dev = nullptr;
     B2_TRY(stage_in(ctx, ctx->stage_in, a, sizeof(Fr) * n, &a_dev));
-    bool q_is_dev = is_device_ptr(q);
-    Fr* q_dev = (Fr*)q;
     size_t qbytes = sizeof(Fr) * (n - 1);
-    if (!q_is_dev) {
-        B2_TRY(scratch_reserve(ctx, ctx->stage_out, qbytes));
-        q_dev = (Fr*)ctx->stage_out.p;
-    }
-    B2_TRY(kate_division(ctx, q_dev, (const Fr*)a_dev, n, b));
-    if (!q_is_dev) return d2h(ctx, q, q_dev, qbytes);
-    return B200ZK_OK;
+    void* q_dev = nullptr;
+    B2_TRY(out_begin(ctx, q, qbytes, &q_dev));
+    B2_TRY(kate_division(ctx, (Fr*)q_dev, (const Fr*)a_dev, n, b));
+    return out_end(ctx, q, q_dev, qbytes);
 }
 
 // ---- diagnostics -----------------------------------------------------------------------------------
@@ -781,9 +695,7 @@ int32_t b200zk_debug_field_op(b200zk_ctx* ctx, int field, int op, void* r, const
     const void *a_dev = nullptr, *b_dev = nullptr;
     B2_TRY(stage_in(ctx, ctx->stage_in, a, bytes, &a_dev));
     B2_TRY(stage_in(ctx, ctx->ntt_work, b, bytes, &b_dev));
-    B2_TRY(scratch_reserve(ctx, ctx->stage_out, bytes));
-    B2_TRY(field_op(ctx, field, op, ctx->stage_out.p, a_dev, b_dev, n));
-    return deliver(ctx, r, ctx->stage_out.p, bytes);
+    return out_small(ctx, r, bytes, [&](void* res) { return field_op(ctx, field, op, res, a_dev, b_dev, n); });
 }
 
 int32_t b200zk_profile_enable(b200zk_ctx* ctx, int on) {

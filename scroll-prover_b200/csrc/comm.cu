@@ -16,9 +16,6 @@
 #include "ec.cuh"
 
 namespace b200zk {
-int32_t msm_run(b200zk_ctx* ctx, const Affine* bases, const Fr* scalars, uint64_t n, Jacobian* out_dev, uint32_t pre_c,
-                uint64_t pre_stride);
-int32_t g1_sum_run(b200zk_ctx* ctx, const Jacobian* pts, uint64_t count, Jacobian* out_dev);
 
 struct NcclApi {
     void* handle = nullptr;
@@ -156,9 +153,8 @@ int32_t b200zk_allgather_rows(b200zk_ctx* ctx, void* values_dev, uint32_t log_si
 static int32_t msm_range_dev(b200zk_ctx* ctx, const b200zk_srs* srs, const void* scalars, uint64_t first, uint64_t n, Jacobian* res) {
     const void* sc_dev = nullptr;
     if (n) B2_TRY(stage_in(ctx, ctx->stage_in, scalars, sizeof(Fr) * n, &sc_dev));
-    // the precomputed tables 2^(c*w) P_i lie at stride srs->n: a slice of them is the same layout with an offset
-    uint32_t pre_c = (srs->pre_c && n * 16 >= srs->n) ? srs->pre_c : 0;
-    return msm_run(ctx, (const Affine*)srs->dev_bases + first, (const Fr*)sc_dev, n, res, pre_c, srs->n);
+    const Fr* sc = (const Fr*)sc_dev;
+    return msm_srs(ctx, srs, first, &sc, 1, n, res);
 }
 
 int32_t b200zk_msm_g1_range(b200zk_ctx* ctx, const b200zk_srs* srs, const void* scalars, uint64_t first, uint64_t n, void* out_jacobian96) {
@@ -169,10 +165,8 @@ int32_t b200zk_msm_g1_range(b200zk_ctx* ctx, const b200zk_srs* srs, const void* 
         return fail(ctx, B200ZK_E_INVALID, "msm_g1_range: [%llu, +%llu) exceeds the %llu bases", (unsigned long long)first,
                     (unsigned long long)n, (unsigned long long)srs->n);
     Guard g(ctx);
-    B2_TRY(scratch_reserve(ctx, ctx->stage_out, 256));
-    Jacobian* res = (Jacobian*)ctx->stage_out.p;
-    B2_TRY(msm_range_dev(ctx, srs, scalars, first, n, res));
-    return deliver(ctx, out_jacobian96, res, sizeof(Jacobian));
+    return out_small(ctx, out_jacobian96, sizeof(Jacobian),
+                     [&](void* res) { return msm_range_dev(ctx, srs, scalars, first, n, (Jacobian*)res); });
 }
 
 int32_t b200zk_msm_g1_sharded(b200zk_ctx* ctx, const b200zk_srs* srs, const void* scalars_slice, uint64_t n_total, void* out_jacobian96) {
@@ -186,12 +180,9 @@ int32_t b200zk_msm_g1_sharded(b200zk_ctx* ctx, const b200zk_srs* srs, const void
     shard_range(n_total, ctx->comm_rank, ctx->comm_world, &first, &cnt);
     if (cnt && !scalars_slice) return fail(ctx, B200ZK_E_INVALID, "msm_g1_sharded: null scalar slice");
     Guard g(ctx);
-    if (ctx->comm_world == 1) {
-        B2_TRY(scratch_reserve(ctx, ctx->stage_out, 256));
-        Jacobian* res = (Jacobian*)ctx->stage_out.p;
-        B2_TRY(msm_range_dev(ctx, srs, scalars_slice, 0, n_total, res));
-        return deliver(ctx, out_jacobian96, res, sizeof(Jacobian));
-    }
+    if (ctx->comm_world == 1)
+        return out_small(ctx, out_jacobian96, sizeof(Jacobian),
+                         [&](void* res) { return msm_range_dev(ctx, srs, scalars_slice, 0, n_total, (Jacobian*)res); });
     NcclApi* api = nccl_api();
     Jacobian* buf = (Jacobian*)ctx->comm_buf;  // [0 .. world) gathered partials, [world] this rank's partial / the sum
     Jacobian* mine = buf + ctx->comm_world;

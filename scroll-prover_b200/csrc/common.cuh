@@ -44,7 +44,7 @@ struct b200zk_srs {
     uint64_t n;
     uint32_t tag;
     uint32_t pre_c;   // 0: plain bases; else window bits the 2^(c*w) tables were built for
-    uint32_t pre_W;
+    uint32_t pre_W;   // dev_bases, pre_c and pre_W belong to msm.cu (srs_init / msm_srs)
 };
 
 struct b200zk_ctx {
@@ -261,11 +261,47 @@ inline int32_t deliver(b200zk_ctx* ctx, void* dst, const void* dev_src, size_t b
     return d2h(ctx, dst, dev_src, bytes);
 }
 
+// An output of `bytes` for `dst`: out_begin hands out dst itself when it is device memory, else stage_out; out_end copies
+// the staged result back to the host.
+inline int32_t out_begin(b200zk_ctx* ctx, void* dst, size_t bytes, void** dev) {
+    if (is_device_ptr(dst)) {
+        *dev = dst;
+        return B200ZK_OK;
+    }
+    B2_TRY(scratch_reserve(ctx, ctx->stage_out, bytes));
+    *dev = ctx->stage_out.p;
+    return B200ZK_OK;
+}
+inline int32_t out_end(b200zk_ctx* ctx, void* dst, const void* dev, size_t bytes) {
+    return dev == dst ? B200ZK_OK : d2h(ctx, dst, dev, bytes);
+}
+
+// A result that is always staged: compute(res) writes it into stage_out (>= 256 B, enough for a point or a field
+// element), then it is delivered to dst.
+template <class F>
+inline int32_t out_small(b200zk_ctx* ctx, void* dst, size_t bytes, F&& compute) {
+    B2_TRY(scratch_reserve(ctx, ctx->stage_out, bytes > 256 ? bytes : 256));
+    B2_TRY(compute(ctx->stage_out.p));
+    return deliver(ctx, dst, ctx->stage_out.p, bytes);
+}
+
 // implemented in ntt.cu / msm.cu / poly.cu
 int32_t ntt_get_table(b200zk_ctx* ctx, const Fr& omega, uint32_t log_n, const Fr** out);
 Fr host_zeta();
 int32_t comm_destroy(b200zk_ctx* ctx);  // comm.cu
 int32_t ntt_run(b200zk_ctx* ctx, const Fr* in, uint32_t log_in, Fr* out, uint32_t log_n, const Fr& omega,
                 int inverse_scale, int coset_mode);
+struct Affine;
+struct Jacobian;
+// srs_init: uploads s->n bases and, for a handle of >= 2^16 bases when device memory allows, builds the precomputed
+// window tables; on failure nothing stays allocated.  msm_srs: cols[0 .. count) of n scalars over the bases
+// [first, first + n) -> out_dev[0 .. count), in pipelines of at most msm_srs_max_batch(s, n) columns.
+int32_t srs_init(b200zk_ctx* ctx, b200zk_srs* s, const void* g1_affine);
+void srs_free(b200zk_srs* s);
+uint32_t msm_srs_max_batch(const b200zk_srs* s, uint64_t n);
+int32_t msm_srs(b200zk_ctx* ctx, const b200zk_srs* s, uint64_t first, const Fr* const* cols, uint32_t count, uint64_t n,
+                Jacobian* out_dev);
+int32_t msm_bases(b200zk_ctx* ctx, const Affine* bases, const Fr* scalars, uint64_t n, Jacobian* out_dev);
+int32_t g1_sum_run(b200zk_ctx* ctx, const Jacobian* pts, uint64_t count, Jacobian* out_dev);
 
 }  // namespace b200zk

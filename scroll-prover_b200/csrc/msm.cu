@@ -558,7 +558,7 @@ __global__ void __launch_bounds__(128) srs_shift_kernel(const Affine* __restrict
     out[i] = xyzz_to_affine(p);
 }
 
-uint32_t msm_pick_window_precomputed(uint64_t n) {
+static uint32_t pick_window_precomputed(uint64_t n) {
     double best = 1e300;
     uint32_t bc = 10;
     for (uint32_t c = 8; c <= 23; ++c) {
@@ -576,7 +576,7 @@ uint32_t msm_pick_window_precomputed(uint64_t n) {
 }
 
 // tables[w] = 2^(c*w) * bases, w = 0..W-1, laid out back to back (stride n); tables[0] must already hold the bases
-int32_t srs_precompute_run(b200zk_ctx* ctx, Affine* tables, uint64_t n, uint32_t c, uint32_t W) {
+static int32_t srs_precompute_run(b200zk_ctx* ctx, Affine* tables, uint64_t n, uint32_t c, uint32_t W) {
     for (uint32_t w = 1; w < W; ++w) {
         srs_shift_kernel<<<(uint32_t)((n + 127) / 128), 128, 0, ctx->stream>>>(tables + (uint64_t)(w - 1) * n, tables + (uint64_t)w * n, n, c);
         B2_LAUNCH_CHECK(ctx);
@@ -585,7 +585,7 @@ int32_t srs_precompute_run(b200zk_ctx* ctx, Affine* tables, uint64_t n, uint32_t
 }
 
 // how many columns of n scalars one batched pipeline may take (sorted-entry positions are 32-bit; scratch stays ~2 GiB)
-uint32_t msm_max_batch(uint64_t n, uint32_t pre_c) {
+static uint32_t msm_max_batch(uint64_t n, uint32_t pre_c) {
     uint32_t c = pre_c ? pre_c : pick_window(n);
     uint64_t per_col = (n ? n : 1) * (254 / c + 1);
     uint64_t b = (1ull << 28) / per_col;
@@ -594,8 +594,8 @@ uint32_t msm_max_batch(uint64_t n, uint32_t pre_c) {
 
 // pre_c != 0: `bases` is a precomputed SRS (W tables of stride pre_stride) built for window pre_c.
 // cols[0 .. batch): device pointers of `batch` scalar vectors of n elements each; out_dev[0 .. batch).
-int32_t msm_run_batch(b200zk_ctx* ctx, const Affine* bases, const Fr* const* cols, uint32_t batch, uint64_t n, Jacobian* out_dev,
-                      uint32_t pre_c, uint64_t pre_stride) {
+static int32_t msm_run_batch(b200zk_ctx* ctx, const Affine* bases, const Fr* const* cols, uint32_t batch, uint64_t n, Jacobian* out_dev,
+                             uint32_t pre_c, uint64_t pre_stride) {
     if (n >= (1ull << 31)) return fail(ctx, B200ZK_E_UNSUPPORTED, "msm: n = %llu >= 2^31", (unsigned long long)n);
     if (batch < 1 || batch > (uint32_t)MSM_MAX_BATCH) return fail(ctx, B200ZK_E_INVALID, "msm: batch %u out of range [1,%d]", batch, MSM_MAX_BATCH);
     MsmPlan pl;
@@ -749,9 +749,71 @@ int32_t msm_run_batch(b200zk_ctx* ctx, const Affine* bases, const Fr* const* col
     return B200ZK_OK;
 }
 
-int32_t msm_run(b200zk_ctx* ctx, const Affine* bases, const Fr* scalars, uint64_t n, Jacobian* out_dev, uint32_t pre_c,
-                uint64_t pre_stride) {
-    return msm_run_batch(ctx, bases, &scalars, 1, n, out_dev, pre_c, pre_stride);
+int32_t msm_bases(b200zk_ctx* ctx, const Affine* bases, const Fr* scalars, uint64_t n, Jacobian* out_dev) {
+    return msm_run_batch(ctx, bases, &scalars, 1, n, out_dev, 0, 0);
+}
+
+// ---- the SRS handle's device side: this file alone reads dev_bases, pre_c and pre_W ---------------------------------
+int32_t srs_init(b200zk_ctx* ctx, b200zk_srs* s, const void* g1_affine) {
+    const uint64_t n = s->n;
+    s->dev_bases = nullptr;
+    s->pre_c = 0;
+    s->pre_W = 1;
+    size_t bytes = sizeof(Affine) * (n ? n : 1);
+    if (ctx->srs_precompute && n >= (1ull << 16)) {
+        // keep 2^(c*w) * P_i for every window w: all windows then share ONE bucket set (no per-window reduction, no
+        // Horner doublings) and a wider window pays off.  Costs W x the base storage; skipped when memory is short.
+        uint32_t c = pick_window_precomputed(n), W = 254 / c + 1;
+        size_t free_b = 0, total_b = 0;
+        if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && (double)bytes * W < 0.35 * (double)free_b) {
+            s->pre_c = c;
+            s->pre_W = W;
+            bytes *= W;
+        }
+    }
+    cudaError_t e = cudaMalloc(&s->dev_bases, bytes);
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        s->dev_bases = nullptr;
+        return fail(ctx, B200ZK_E_OOM, "srs_register: cudaMalloc(%zu) failed", bytes);
+    }
+    cudaMemcpyKind kind = is_device_ptr(g1_affine) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    e = n ? cudaMemcpyAsync(s->dev_bases, g1_affine, sizeof(Affine) * n, kind, ctx->stream) : cudaSuccess;
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) {
+        srs_free(s);
+        return fail(ctx, B200ZK_E_CUDA, "srs_register: upload failed: %s", cudaGetErrorString(e));
+    }
+    if (s->pre_c) {
+        int32_t rc = srs_precompute_run(ctx, (Affine*)s->dev_bases, n, s->pre_c, s->pre_W);
+        if (rc == B200ZK_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = B200ZK_E_CUDA;
+        if (rc != B200ZK_OK) {
+            srs_free(s);
+            return fail(ctx, rc, "srs_register: precomputation failed");
+        }
+    }
+    return B200ZK_OK;
+}
+
+void srs_free(b200zk_srs* s) {
+    if (s->dev_bases) cudaFree(s->dev_bases);
+    s->dev_bases = nullptr;
+}
+
+// a commit over a short prefix of a large precomputed SRS is cheaper with the plain bases (table 0) and a window sized for n
+// than with the handle's wide window (2^(c-1) buckets to reduce)
+static uint32_t srs_pre_c(const b200zk_srs* s, uint64_t n) { return (s->pre_c && n * 16 >= s->n) ? s->pre_c : 0; }
+
+uint32_t msm_srs_max_batch(const b200zk_srs* s, uint64_t n) { return msm_max_batch(n, srs_pre_c(s, n)); }
+
+int32_t msm_srs(b200zk_ctx* ctx, const b200zk_srs* s, uint64_t first, const Fr* const* cols, uint32_t count, uint64_t n,
+                Jacobian* out_dev) {
+    const uint32_t pre_c = srs_pre_c(s, n), bmax = msm_max_batch(n, pre_c);
+    // the precomputed tables 2^(c*w) P_i lie at stride s->n: a slice of them is the same layout with an offset
+    const Affine* bases = (const Affine*)s->dev_bases + first;
+    for (uint32_t j = 0; j < count; j += bmax)
+        B2_TRY(msm_run_batch(ctx, bases, cols + j, count - j < bmax ? count - j : bmax, n, out_dev + j, pre_c, s->n));
+    return B200ZK_OK;
 }
 
 int32_t g1_sum_run(b200zk_ctx* ctx, const Jacobian* pts, uint64_t count, Jacobian* out_dev) {
