@@ -149,6 +149,21 @@ B200ZK_API int32_t b200zk_ntt_fr(b200zk_ctx* ctx, void* data, uint32_t log_n, co
 B200ZK_API int32_t b200zk_ntt_fr_ext(b200zk_ctx* ctx, const void* in, uint32_t log_in, void* out, uint32_t log_n,
                           const void* omega32, int inverse_scale, int coset_mode);
 
+/* ---- coset parts of the extended domain ------------------------------------------------------- */
+/* With n = 2^k, J = 2^(extended_k - k) and w = extended_omega^J, the extended coset zeta*<extended_omega> is the union of
+ * the J cosets g_j*<w>, g_j = zeta * extended_omega^j, and extended index j + J*r is row r of part j.  evaluate_h can
+ * then hold one part (n values) per column instead of the whole coset (J*n).  2 <= J <= 16, else B200ZK_E_UNSUPPORTED;
+ * part >= J is B200ZK_E_INVALID.  Pointers are host or device memory. */
+/* out[r] = coeff_to_extended(a)[part + J*r], r < 2^k: a (2^k coefficients) evaluated at zeta*extended_omega^part*omega^r.
+ * coeffs == out is allowed. */
+B200ZK_API int32_t b200zk_coeff_to_extended_part(b200zk_ctx* ctx, const void* coeffs, uint32_t k, uint32_t extended_k,
+                                                 const void* extended_omega32, uint32_t part, void* out);
+/* parts[j] (J vectors of 2^k) = evaluations on coset part j -> in place, parts[t] = coefficients [t*2^k, (t+1)*2^k) of
+ * extended_to_coeff(interleave(parts)) before truncation; divide_by_vanishing != 0 divides by X^n - 1 first
+ * (divide_by_vanishing_poly). */
+B200ZK_API int32_t b200zk_extended_parts_to_coeff(b200zk_ctx* ctx, void* const* parts, uint32_t k, uint32_t extended_k,
+                                                  const void* extended_omega32, int divide_by_vanishing);
+
 /* ---- device-resident column pipeline (the per-column work of plonk::create_proof) ---------------- */
 /* For each of `count` columns of 2^k Lagrange values in HOST memory (pinned => the H2D copy of column j+1 overlaps the
  * kernels of column j on an internal copy stream; pageable works too):
@@ -305,6 +320,15 @@ B200ZK_API int32_t b200zk_graph_evaluate_rows(b200zk_ctx* ctx, const b200zk_grap
                                               uint32_t n_challenges, const void* beta32, const void* gamma32, const void* theta32,
                                               const void* y32, const void* extended_omega32, void* values_dev, uint32_t log_size,
                                               int32_t rot_scale, uint64_t row_first, uint64_t row_count);
+/* b200zk_graph_evaluate on coset part `part` of the extended domain (see b200zk_coeff_to_extended_part): columns and values
+ * are the 2^k values of that part, rotations read (r + rotation) mod 2^k, ExtendedX = zeta * extended_omega^part * w^r.
+ * values[r] then equals what b200zk_graph_evaluate over the whole coset (rot_scale = J) leaves at row part + J*r. */
+B200ZK_API int32_t b200zk_graph_evaluate_part(b200zk_ctx* ctx, const b200zk_graph* graph, const void* const* fixed_dev,
+                                              uint32_t n_fixed, const void* const* advice_dev, uint32_t n_advice,
+                                              const void* const* instance_dev, uint32_t n_instance, const void* challenges32,
+                                              uint32_t n_challenges, const void* beta32, const void* gamma32, const void* theta32,
+                                              const void* y32, const void* extended_omega32, void* values_dev, uint32_t k,
+                                              uint32_t extended_k, uint32_t part);
 /* Collective over the context's communicator: values_dev holds 2^log_size field elements of which this rank has written its
  * b200zk_shard_range(2^log_size, rank, world) slice; afterwards every rank holds all slices (one in-place ncclAllGather of the
  * 32-byte elements over NVLink, on the context stream).  world must divide 2^log_size (a power of two); world == 1 is a no-op. */

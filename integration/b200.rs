@@ -84,6 +84,34 @@ pub(crate) fn extended_to_coeff(values: &mut [Fr], extended_k: u32, extended_ome
     check(unsafe { sys::b200zk_ntt_fr(ctx(), values.as_mut_ptr() as _, extended_k, p(&extended_omega_inv), 1, sys::COSET_POST) });
 }
 
+/// Part `part` of the extended coset (J = 2^(extended_k - k) parts): out[r] = coeff_to_extended(coeffs)[part + J*r]
+pub(crate) fn coeff_to_extended_part(coeffs: &[Fr], k: u32, extended_k: u32, extended_omega: Fr, part: u32, out: &mut [Fr]) {
+    assert_eq!(coeffs.len(), 1 << k);
+    assert_eq!(out.len(), 1 << k);
+    check(unsafe {
+        sys::b200zk_coeff_to_extended_part(ctx(), coeffs.as_ptr() as _, k, extended_k, p(&extended_omega), part, out.as_mut_ptr() as _)
+    });
+}
+/// parts[j] = values on coset part j -> in place, parts[t] = coefficients [t*n, (t+1)*n) of extended_to_coeff of the
+/// interleaved coset (before the truncation), divided by X^n - 1 first when `divide_by_vanishing`
+pub(crate) fn extended_parts_to_coeff(parts: &mut [Vec<Fr>], k: u32, extended_k: u32, extended_omega: Fr, divide_by_vanishing: bool) {
+    assert_eq!(parts.len(), 1 << (extended_k - k));
+    let ptrs: Vec<*mut c_void> = parts.iter_mut().map(|v| { assert_eq!(v.len(), 1 << k); v.as_mut_ptr() as _ }).collect();
+    check(unsafe {
+        sys::b200zk_extended_parts_to_coeff(ctx(), ptrs.as_ptr(), k, extended_k, p(&extended_omega), divide_by_vanishing as i32)
+    });
+}
+/// GraphEvaluator::evaluate on coset part `part`: device columns and values of 2^k elements each (that part's rows)
+pub(crate) fn graph_evaluate_part(graph: *const sys::Graph, fixed_dev: &[*const c_void], advice_dev: &[*const c_void],
+                                  instance_dev: &[*const c_void], challenges: &[Fr], beta: Fr, gamma: Fr, theta: Fr, y: Fr,
+                                  extended_omega: Fr, values_dev: *mut c_void, k: u32, extended_k: u32, part: u32) {
+    check(unsafe {
+        sys::b200zk_graph_evaluate_part(ctx(), graph, fixed_dev.as_ptr(), fixed_dev.len() as u32, advice_dev.as_ptr(), advice_dev.len() as u32,
+                                        instance_dev.as_ptr(), instance_dev.len() as u32, challenges.as_ptr() as _, challenges.len() as u32,
+                                        p(&beta), p(&gamma), p(&theta), p(&y), p(&extended_omega), values_dev, k, extended_k, part)
+    });
+}
+
 pub(crate) fn eval_polynomial(poly: &[Fr], point: Fr) -> Fr {
     let mut out = Fr::zero();
     check(unsafe { sys::b200zk_eval_poly(ctx(), poly.as_ptr() as _, poly.len() as u64, p(&point), &mut out as *mut Fr as _) });

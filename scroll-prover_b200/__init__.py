@@ -82,6 +82,8 @@ def _signatures():
         "b200zk_g_to_lagrange": [vp, vp, u32, vp],
         "b200zk_ntt_fr": [vp, vp, u32, vp, C.c_int, C.c_int],
         "b200zk_ntt_fr_ext": [vp, vp, u32, vp, u32, vp, C.c_int, C.c_int],
+        "b200zk_coeff_to_extended_part": [vp, vp, u32, u32, vp, u32, vp],
+        "b200zk_extended_parts_to_coeff": [vp, C.POINTER(vp), u32, u32, vp, C.c_int],
         "b200zk_ctx_set_overlap": [vp, C.c_int],
         "b200zk_run_column_jobs": [vp, vp, u32, u32, vp, vp, vp, u32, vp],
         "b200zk_commit_columns": [vp, vp, C.POINTER(vp), u32, u32, vp, vp, u32, vp, C.POINTER(vp), C.POINTER(vp), C.c_int],
@@ -106,6 +108,8 @@ def _signatures():
                                   vp, u32, i32],
         "b200zk_graph_evaluate_rows": [vp, vp, C.POINTER(vp), u32, C.POINTER(vp), u32, C.POINTER(vp), u32, vp, u32, vp, vp, vp, vp, vp,
                                        vp, u32, i32, u64, u64],
+        "b200zk_graph_evaluate_part": [vp, vp, C.POINTER(vp), u32, C.POINTER(vp), u32, C.POINTER(vp), u32, vp, u32, vp, vp, vp, vp, vp,
+                                       vp, u32, u32, u32],
         "b200zk_allgather_rows": [vp, vp, u32],
         "b200zk_debug_field_op": [vp, C.c_int, C.c_int, vp, vp, vp, u64],
         "b200zk_profile_enable": [vp, C.c_int],
@@ -634,6 +638,25 @@ class Graph:
             self.ctx._ck(lib().b200zk_graph_evaluate_rows(*args, rows[0], rows[1]))
         return values
 
+    def evaluate_part(self, values, k: int, extended_k: int, part: int, fixed=(), advice=(), instance=(), challenges=None, beta=None,
+                      gamma=None, theta=None, y=None, extended_omega=None):
+        """b200zk_graph_evaluate_part: evaluate on coset part `part` of the extended domain; values and every column hold the
+        2^k values of that part (device memory), and values[r] ends up as evaluate() over the whole coset (rot_scale =
+        2^(extended_k - k)) leaves row part + J*r."""
+        assert _count(values, 32) == 1 << k
+        zero = np.zeros(4, np.uint64)
+        tf, kf = Context._dev_table(fixed)
+        ta, ka = Context._dev_table(advice)
+        ti, ki = Context._dev_table(instance)
+        ch = np.ascontiguousarray(np.asarray(challenges if challenges is not None else [], dtype=np.uint64).reshape(-1, 4))
+        sc = [_ptr(zero if v is None else v) for v in (beta, gamma, theta, y)]
+        pw, kw = _ptr(extended_omega)
+        pv, kv = _ptr(values)
+        self.ctx._ck(lib().b200zk_graph_evaluate_part(self.ctx._h, self._h, tf, len(fixed), ta, len(advice), ti, len(instance),
+                                                      C.c_void_p(ch.ctypes.data) if len(ch) else None, len(ch), *[p for p, _ in sc],
+                                                      pw, pv, k, extended_k, part))
+        return values
+
     def release(self):
         if self._h:
             lib().b200zk_graph_destroy(self.ctx._h, self._h)
@@ -756,6 +779,34 @@ class EvaluationDomain:
             else:
                 out = np.zeros((1 << self.extended_k, 4), np.uint64)
         return self.ctx.ntt_ext(a, self.k, out, self.extended_k, self.extended_omega, False, COSET_PRE)
+
+    @property
+    def n_parts(self) -> int:
+        """J = 2^(extended_k - k): the number of size-n cosets the extended coset splits into."""
+        return 1 << (self.extended_k - self.k)
+
+    def coeff_to_extended_part(self, a, part: int, out=None):
+        """out[r] = coeff_to_extended(a)[part + J*r] for r < n, computed with one size-n transform (a may be out)."""
+        if out is None:
+            out = _like(a)
+        assert _count(a, 32) == self.n and _count(out, 32) == self.n
+        pa, k1 = _ptr(a)
+        po, k2 = _ptr(out)
+        pw, k3 = _ptr(self.extended_omega)
+        self.ctx._ck(lib().b200zk_coeff_to_extended_part(self.ctx._h, pa, self.k, self.extended_k, pw, part, po))
+        return _write_back(out, k2)
+
+    def extended_parts_to_coeff(self, parts, divide_by_vanishing: bool = False):
+        """In place: parts[j] holds the values on coset part j; afterwards parts[t] holds coefficients [t*n, (t+1)*n) of
+        extended_to_coeff (before its truncation) of the interleaved coset, divided by X^n - 1 first when asked."""
+        assert len(parts) == self.n_parts and all(_count(p, 32) == self.n for p in parts)
+        keep = [_ptr(p) for p in parts]
+        arr = (C.c_void_p * len(parts))(*[p.value for p, _ in keep])
+        pw, kw = _ptr(self.extended_omega)
+        self.ctx._ck(lib().b200zk_extended_parts_to_coeff(self.ctx._h, arr, self.k, self.extended_k, pw, int(divide_by_vanishing)))
+        for p, (_, kp) in zip(parts, keep):
+            _write_back(p, kp)
+        return parts
 
     def extended_to_coeff(self, a):
         """ifft(extended_omega_inv) + distribute_powers_zeta(out of coset); returns the first n*(j-1) coefficients."""

@@ -349,6 +349,66 @@ int32_t b200zk_ntt_fr(b200zk_ctx* ctx, void* data, uint32_t log_n, const void* o
     return b200zk_ntt_fr_ext(ctx, data, log_n, data, log_n, omega32, inverse_scale, coset_mode);
 }
 
+// ---- coset parts of the extended domain ---------------------------------------------------------
+int32_t b200zk_coeff_to_extended_part(b200zk_ctx* ctx, const void* coeffs, uint32_t k, uint32_t extended_k,
+                                      const void* extended_omega32, uint32_t part, void* out) {
+    CHECK_CTX(ctx);
+    if (!coeffs || !out || !extended_omega32) return fail(ctx, B200ZK_E_INVALID, "coeff_to_extended_part: null pointer");
+    B2_TRY(check_part(ctx, k, extended_k, part, "coeff_to_extended_part"));
+    Guard g(ctx);
+    Fr we;
+    B2_TRY(read_fr(ctx, extended_omega32, &we));
+    const size_t bytes = sizeof(Fr) << k;
+    void* out_dev = nullptr;
+    B2_TRY(out_begin(ctx, out, bytes, &out_dev));
+    const void* in_dev = nullptr;
+    if (!is_device_ptr(coeffs) && out_dev != out) {  // host in / host out: upload into the output staging, run in place
+        B2_TRY(h2d(ctx, out_dev, coeffs, bytes));
+        in_dev = out_dev;
+    } else {
+        B2_TRY(stage_in(ctx, ctx->stage_in, coeffs, bytes, &in_dev));
+    }
+    B2_TRY(ntt_run_part(ctx, (const Fr*)in_dev, (Fr*)out_dev, k, extended_k, we, part, false, Fr::one()));
+    return out_end(ctx, out, out_dev, bytes);
+}
+
+int32_t b200zk_extended_parts_to_coeff(b200zk_ctx* ctx, void* const* parts, uint32_t k, uint32_t extended_k,
+                                       const void* extended_omega32, int divide_by_vanishing) {
+    CHECK_CTX(ctx);
+    if (!parts || !extended_omega32) return fail(ctx, B200ZK_E_INVALID, "extended_parts_to_coeff: null pointer");
+    B2_TRY(check_part(ctx, k, extended_k, 0, "extended_parts_to_coeff"));
+    const uint32_t J = 1u << (extended_k - k);
+    for (uint32_t j = 0; j < J; ++j)
+        if (!parts[j]) return fail(ctx, B200ZK_E_INVALID, "extended_parts_to_coeff: parts[%u] is null", j);
+    Guard g(ctx);
+    Fr we;
+    B2_TRY(read_fr(ctx, extended_omega32, &we));
+    const uint64_t n = 1ull << k;
+    const size_t bytes = sizeof(Fr) * n;
+    // device parts are transformed where they are; host parts go through slot j of stage_out and back
+    bool host[16];
+    uint32_t n_host = 0;
+    for (uint32_t j = 0; j < J; ++j) n_host += (host[j] = !is_device_ptr(parts[j]));
+    if (n_host) B2_TRY(scratch_reserve(ctx, ctx->stage_out, bytes * J));
+    Fr* dp[16];
+    for (uint32_t j = 0; j < J; ++j) {
+        dp[j] = host[j] ? (Fr*)((char*)ctx->stage_out.p + bytes * j) : (Fr*)parts[j];
+        if (host[j]) B2_TRY(h2d(ctx, dp[j], parts[j], bytes));
+    }
+    // part j: inverse transform with post-scale n^-1 g_j^-i, times (g_j^n - 1)^-1 (X^n - 1 is that constant on the part)
+    const Fr one = Fr::one(), wn = we.pow_u64(n);
+    Fr gjn = host_zeta().pow_u64(n);
+    for (uint32_t j = 0; j < J; ++j) {
+        const Fr scale = divide_by_vanishing ? (gjn - one).inv() : one;
+        B2_TRY(ntt_run_part(ctx, dp[j], dp[j], k, extended_k, we, j, true, scale));
+        gjn = gjn * wn;
+    }
+    B2_TRY(parts_idft_run(ctx, dp, k, extended_k, we));
+    for (uint32_t j = 0; j < J; ++j)
+        if (host[j]) B2_TRY(d2h(ctx, parts[j], dp[j], bytes));
+    return B200ZK_OK;
+}
+
 // ---- device-resident column pipeline (SURVEY.md §8(f).1) -------------------------------------------
 static int32_t pipeline_init(b200zk_ctx* ctx) {
     if (ctx->copy_stream) return B200ZK_OK;

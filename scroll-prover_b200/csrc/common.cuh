@@ -291,6 +291,17 @@ Fr host_zeta();
 int32_t comm_destroy(b200zk_ctx* ctx);  // comm.cu
 int32_t ntt_run(b200zk_ctx* ctx, const Fr* in, uint32_t log_in, Fr* out, uint32_t log_n, const Fr& omega,
                 int inverse_scale, int coset_mode);
+// coset parts of the extended domain (ntt.cu / quotient.cu): J = 2^(log_N - k) parts of 2^k points, part j = g_j<w>
+int32_t ntt_run_part(b200zk_ctx* ctx, const Fr* in, Fr* out, uint32_t k, uint32_t log_N, const Fr& ext_omega, uint32_t part,
+                     bool inverse, const Fr& scale);
+int32_t parts_idft_run(b200zk_ctx* ctx, Fr* const* parts, uint32_t k, uint32_t log_N, const Fr& ext_omega);
+inline int32_t check_part(b200zk_ctx* ctx, uint32_t k, uint32_t extended_k, uint32_t part, const char* what) {
+    if (extended_k <= k || extended_k - k > 4 || extended_k > 28)
+        return fail(ctx, B200ZK_E_UNSUPPORTED, "%s: J = 2^(extended_k - k) with k = %u, extended_k = %u: only 2 <= J <= 16", what, k,
+                    extended_k);
+    if (part >= (1u << (extended_k - k))) return fail(ctx, B200ZK_E_INVALID, "%s: part %u >= J = %u", what, part, 1u << (extended_k - k));
+    return B200ZK_OK;
+}
 struct Affine;
 struct Jacobian;
 // srs_init: uploads s->n bases and, for a handle of >= 2^16 bases when device memory allows, builds the precomputed

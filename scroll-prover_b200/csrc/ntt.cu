@@ -18,6 +18,11 @@
 // shared by every domain size under the same root (w_{2^u} = ROOT_OF_UNITY^(2^(28-u)) for all k).
 // Fused: zero padding + zeta^i coset pre-scaling on load (coeff_to_extended), n^-1 and zeta^-i
 // post-scaling on the final store (ifft / extended_to_coeff).
+// Coset parts (PART = true, ntt_run_part): the extended coset zeta<w_ext> of 2^extended_k points is the union of the
+// J = 2^(extended_k - k) cosets g_j<w> of the base domain, g_j = zeta * w_ext^j, w = w_ext^J (extended index j + J*r is
+// row r of part j).  A part is a size-2^k transform with the pre-scale g_j^i = zeta^(i mod 3) * w_ext^(j*i) on load, or
+// the inverse with the post-scale g_j^-i on store; w_ext^e comes from the top level of the extended table,
+// w_ext^(e + N/2) = -w_ext^e.
 #include "common.cuh"
 
 namespace b200zk {
@@ -71,6 +76,19 @@ __device__ __forceinline__ void st_fr(Fr* p, const Fr& r) {
     q[0] = make_uint4(r.l.v[0], r.l.v[1], r.l.v[2], r.l.v[3]);
     q[1] = make_uint4(r.l.v[4], r.l.v[5], r.l.v[6], r.l.v[7]);
 }
+// PART kernels: etab = the top level of the 2^log_N table of w_ext (w_ext^e, e < N/2); pass 0 multiplies coefficient i by
+// w_ext^(j*i) when ps.pre, the last pass multiplies output i by w_ext^(-j*i) when ps.post
+struct PartTw {
+    const Fr* etab;
+    uint32_t j, log_N;
+};
+
+__device__ __forceinline__ Fr ext_pow(const PartTw& pt, uint32_t e) {  // w_ext^e, e < N
+    const uint32_t half = 1u << (pt.log_N - 1);
+    Fr w = ldg_fr(pt.etab + (e & (half - 1)));
+    return e >= half ? Fr::zero() - w : w;
+}
+
 __device__ __forceinline__ Fr ld_sm(const uint4* lo, const uint4* hi, uint32_t i) {
     uint4 a = lo[i], b = hi[i];
     Fr r;
@@ -104,10 +122,10 @@ __global__ void ntt_build_table(Fr* tab, LevelRoots roots, uint32_t log_n) {
 }
 
 // One pass over one tile.  C = lanes per tile (8, or 1 for the single-pass small transform).
-template <int C, bool LAST>
+template <int C, bool LAST, bool PART>
 __global__ void __launch_bounds__(NTT_THREADS, 3)
 ntt_pass_kernel(const Fr* __restrict__ in, Fr* __restrict__ out, const Fr* __restrict__ tab, NttPass ps, Fr3 pre_c,
-                Fr3 post_c) {
+                Fr3 post_c, PartTw pt) {
     extern __shared__ uint4 smem[];
     const uint32_t m = ps.m, L = 1u << m, E = L * C;
     uint4* lo = smem;
@@ -180,6 +198,10 @@ ntt_pass_kernel(const Fr* __restrict__ in, Fr* __restrict__ out, const Fr* __res
             if (ps.p == 0 && ps.pre) {
                 uint32_t r3 = (uint32_t)(gi % 3);
                 if (r3) v = v * sel3(pre_c, r3);
+                if (PART) {  // j * gi < J * 2^k = N: no reduction
+                    uint32_t e = pt.j * (uint32_t)gi;
+                    if (e) v = v * ext_pow(pt, e);
+                }
             }
         }
         uint32_t pos = __brev(d) >> (32 - m);
@@ -267,7 +289,13 @@ ntt_pass_kernel(const Fr* __restrict__ in, Fr* __restrict__ out, const Fr* __res
             go = base + ((uint64_t)K << rest) + lane;
         } else {
             go = ((uint64_t)K << t) + c + lane;
-            if (ps.post) v = v * sel3(post_c, (uint32_t)(go % 3));
+            if (ps.post) {
+                v = v * sel3(post_c, (uint32_t)(go % 3));
+                if (PART) {
+                    uint32_t e = (0u - pt.j * (uint32_t)go) & ((1u << pt.log_N) - 1);
+                    if (e) v = v * ext_pow(pt, e);
+                }
+            }
         }
         st_fr(out + go, v);
     }
@@ -363,14 +391,14 @@ static void plan_digits(uint32_t log_n, uint32_t* P, uint32_t dig[4]) {
     for (uint32_t i = 0; i < 4; ++i) dig[i] = (i < p) ? basebits + (i < extra ? 1 : 0) : 0;
 }
 
-template <int C, bool LAST>
+template <int C, bool LAST, bool PART>
 static int32_t launch_pass(b200zk_ctx* ctx, const Fr* in, Fr* out, const Fr* tab, const NttPass& ps, const Fr3& pre_c,
-                           const Fr3& post_c) {
+                           const Fr3& post_c, const PartTw& pt) {
     uint32_t L = 1u << ps.m, E = L * C;
     size_t smem = (size_t)(2 * E + (LAST ? 0 : 2 * L)) * sizeof(uint4);
-    const uint32_t optin_bit = 1u << ((C == 8 ? 0 : 2) + (LAST ? 1 : 0));
+    const uint32_t optin_bit = 1u << ((C == 8 ? 0 : 2) + (LAST ? 1 : 0) + (PART ? 4 : 0));
     if (!(ctx->smem_optin & optin_bit)) {
-        B2_CUDA(ctx, cudaFuncSetAttribute(ntt_pass_kernel<C, LAST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        B2_CUDA(ctx, cudaFuncSetAttribute(ntt_pass_kernel<C, LAST, PART>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)((2 * (1u << NTT_MAX_DIGIT) * C + 2 * (1u << NTT_MAX_DIGIT)) * sizeof(uint4))));
         ctx->smem_optin |= optin_bit;
     }
@@ -379,18 +407,21 @@ static int32_t launch_pass(b200zk_ctx* ctx, const Fr* in, Fr* out, const Fr* tab
     uint32_t threads = nb >= NTT_THREADS ? NTT_THREADS : (nb < 32 ? 32 : nb);
     {
         ProfScope psc(ctx, PROF_NTT_PASS);
-        ntt_pass_kernel<C, LAST><<<(uint32_t)tiles, threads, smem, ctx->stream>>>(in, out, tab, ps, pre_c, post_c);
+        ntt_pass_kernel<C, LAST, PART><<<(uint32_t)tiles, threads, smem, ctx->stream>>>(in, out, tab, ps, pre_c, post_c, pt);
     }
     B2_LAUNCH_CHECK(ctx);
     return B200ZK_OK;
 }
 
-int32_t ntt_run(b200zk_ctx* ctx, const Fr* in, uint32_t log_in, Fr* out, uint32_t log_n, const Fr& omega,
-                int inverse_scale, int coset_mode) {
+// part == nullptr: the plain / coset transform.  part != nullptr: a coset-part transform (pre or post per coset_mode, with
+// the zeta^(+-i) factors of pre_c / post_c times w_ext^(+-j*i)); `scale` multiplies the post-scale (vanishing inverse).
+template <bool PART>
+static int32_t ntt_run_impl(b200zk_ctx* ctx, const Fr* in, uint32_t log_in, Fr* out, uint32_t log_n, const Fr& omega,
+                            int inverse_scale, int coset_mode, const PartTw& pt, const Fr& extra_scale) {
     if (log_n > 28) return fail(ctx, B200ZK_E_INVALID, "log_n %u exceeds Fr two-adicity 28", log_n);
     if (log_in > log_n) return fail(ctx, B200ZK_E_INVALID, "log_in %u > log_n %u", log_in, log_n);
     if (coset_mode < 0 || coset_mode > 2) return fail(ctx, B200ZK_E_INVALID, "bad coset_mode %d", coset_mode);
-    if (log_n == 0) {  // length-1 transform is the identity (times 1)
+    if (log_n == 0 && !PART) {  // length-1 transform is the identity (times 1)
         if (in != out) B2_CUDA(ctx, cudaMemcpyAsync(out, in, sizeof(Fr), cudaMemcpyDeviceToDevice, ctx->stream));
         return B200ZK_OK;
     }
@@ -402,7 +433,7 @@ int32_t ntt_run(b200zk_ctx* ctx, const Fr* in, uint32_t log_in, Fr* out, uint32_
     pre_c.c[0] = Fr::one();
     pre_c.c[1] = zeta;
     pre_c.c[2] = zeta2;
-    Fr scale = Fr::one();
+    Fr scale = extra_scale;
     if (inverse_scale)
         for (uint32_t i = 0; i < log_n; ++i) scale = host_halve(scale);
     post_c.c[0] = scale;
@@ -423,7 +454,7 @@ int32_t ntt_run(b200zk_ctx* ctx, const Fr* in, uint32_t log_in, Fr* out, uint32_
         ps.log_in = log_in;
         ps.pre = pre;
         ps.post = post;
-        return launch_pass<1, true>(ctx, in, out, tab, ps, pre_c, post_c);
+        return launch_pass<1, true, PART>(ctx, in, out, tab, ps, pre_c, post_c, pt);
     }
     size_t bytes = sizeof(Fr) << log_n;
     B2_TRY(scratch_reserve(ctx, ctx->ntt_work, bytes));
@@ -438,12 +469,36 @@ int32_t ntt_run(b200zk_ctx* ctx, const Fr* in, uint32_t log_in, Fr* out, uint32_
         ps.pre = (p == 0) ? pre : 0;
         ps.post = (p + 1 == ps.P) ? post : 0;
         if (p + 1 < ps.P)
-            B2_TRY((launch_pass<8, false>(ctx, p == 0 ? in : W, W, tab, ps, pre_c, post_c)));
+            B2_TRY((launch_pass<8, false, PART>(ctx, p == 0 ? in : W, W, tab, ps, pre_c, post_c, pt)));
         else
-            B2_TRY((launch_pass<8, true>(ctx, W, out, tab, ps, pre_c, post_c)));
+            B2_TRY((launch_pass<8, true, PART>(ctx, W, out, tab, ps, pre_c, post_c, pt)));
         t += ps.m;
     }
     return B200ZK_OK;
+}
+
+int32_t ntt_run(b200zk_ctx* ctx, const Fr* in, uint32_t log_in, Fr* out, uint32_t log_n, const Fr& omega,
+                int inverse_scale, int coset_mode) {
+    return ntt_run_impl<false>(ctx, in, log_in, out, log_n, omega, inverse_scale, coset_mode, PartTw{nullptr, 0, 0}, Fr::one());
+}
+
+// Part `part` of the extended coset (J = 2^(log_N - k) parts, w_ext = ext_omega a primitive 2^log_N-th root):
+//   forward: out[r] = sum_i in[i] (g_j w^r)^i,  g_j = zeta * w_ext^j, w = w_ext^J      (in: 2^k coefficients)
+//   inverse: out[i] = scale * n^-1 * g_j^-i * sum_r in[r] w^-ir                       (in: 2^k values on the part)
+// in == out is allowed.
+int32_t ntt_run_part(b200zk_ctx* ctx, const Fr* in, Fr* out, uint32_t k, uint32_t log_N, const Fr& ext_omega, uint32_t part,
+                     bool inverse, const Fr& scale) {
+    if (log_N <= k || log_N > 28 || part >= (1u << (log_N - k)))
+        return fail(ctx, B200ZK_E_INVALID, "ntt_run_part: bad part %u of 2^%u / 2^%u", part, log_N, k);
+    PartTw pt;
+    B2_TRY(ntt_get_table(ctx, ext_omega, log_N, &pt.etab));  // first: the level-k table of w below is the same family
+    pt.etab += 1ull << (log_N - 1);
+    pt.j = part;
+    pt.log_N = log_N;
+    Fr w = ext_omega;
+    for (uint32_t i = k; i < log_N; ++i) w = w.sqr();
+    if (inverse) w = w.inv();
+    return ntt_run_impl<true>(ctx, in, k, out, k, w, inverse ? 1 : 0, inverse ? B200ZK_COSET_POST : B200ZK_COSET_PRE, pt, scale);
 }
 
 }  // namespace b200zk

@@ -384,6 +384,85 @@ int32_t logup_running_sum_run(b200zk_ctx* ctx, const void* const* inputs, uint32
     return prefix_scan_run(ctx, B200ZK_SCAN_SUM, d, n, phi_init, phi_out, (Fr*)(base + o_scan));
 }
 
+// ------------------------------------------------------------------------------------------------ coset parts -> coefficients
+// h has J*n coefficients (n = 2^k); part j of the extended coset is g_j<w>, g_j = zeta * w_ext^j, w = w_ext^J.  After the
+// per-part inverse transform with post-scale g_j^-i (ntt_run_part), part j holds
+//     iNTT_n(e_j)[i] * g_j^-i = sum_t (h_{i+nt} zeta^{nt}) w_J^{jt},   w_J = w_ext^n (a primitive J-th root),
+// because g_j^{nt} = zeta^{nt} w_ext^{jnt}.  So for every i the J values across the parts are a J-point DFT of
+// c_t = h_{i+nt} zeta^{nt}, and h_{i+nt} = J^-1 zeta^{-nt} sum_j part_j[i] w_J^{-jt}: one J-point inverse DFT per i, in
+// place, after which parts[t][i] = h_{i+nt}.  Each thread owns one i: J loads and J stores of 32 B, (J/2) log2 J products
+// of a radix-2 network held in registers plus J scalings -- HBM-bound for the J = 4 of the chunk protocol.
+struct PartsIdft {
+    Fr* parts[16];
+    Fr w[8];   // w_J^-m, m < J/2
+    Fr s[16];  // J^-1 * zeta^(-n*t)
+};
+
+__host__ __device__ constexpr uint32_t brev_bits(uint32_t x, uint32_t bits) {
+    uint32_t r = 0;
+    for (uint32_t b = 0; b < bits; ++b) r |= ((x >> b) & 1u) << (bits - 1 - b);
+    return r;
+}
+
+template <int LOGJ>
+__global__ void __launch_bounds__(256) parts_idft_kernel(PartsIdft P, uint64_t n) {
+    constexpr int J = 1 << LOGJ;
+    uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        Fr a[J];
+#pragma unroll
+        for (int j = 0; j < J; ++j) a[j] = q_ld(P.parts[brev_bits(j, LOGJ)] + i);  // bit-reversed in, natural out
+#pragma unroll
+        for (int len = 2; len <= J; len <<= 1) {
+#pragma unroll
+            for (int b = 0; b < J; b += len) {
+#pragma unroll
+                for (int k = 0; k < len / 2; ++k) {
+                    Fr u = a[b + k], v = a[b + k + len / 2];
+                    if (k) v = v * P.w[k * (J / len)];
+                    a[b + k] = u + v;
+                    a[b + k + len / 2] = u - v;
+                }
+            }
+        }
+#pragma unroll
+        for (int t = 0; t < J; ++t) q_st(P.parts[t] + i, a[t] * P.s[t]);
+    }
+}
+
+// parts[t] (J = 2^(log_N - k) device vectors of 2^k) <- the J-point inverse DFT above; ext_omega a primitive 2^log_N-th root
+int32_t parts_idft_run(b200zk_ctx* ctx, Fr* const* parts, uint32_t k, uint32_t log_N, const Fr& ext_omega) {
+    const uint32_t logj = log_N - k, J = 1u << logj;
+    const uint64_t n = 1ull << k;
+    PartsIdft P;
+    memset(&P, 0, sizeof P);
+    for (uint32_t t = 0; t < J; ++t) P.parts[t] = parts[t];
+    Fr wj_inv = ext_omega.pow_u64(n).inv();  // w_J^-1
+    Fr w = Fr::one();
+    for (uint32_t m = 0; m < J / 2; ++m) {
+        P.w[m] = w;
+        w = w * wj_inv;
+    }
+    Fr jf = Fr::zero();
+    jf.l.v[0] = J;
+    Fr s = jf.to_mont().inv(), zn_inv = host_zeta().pow_u64(n).inv();  // J^-1, zeta^-n
+    for (uint32_t t = 0; t < J; ++t) {
+        P.s[t] = s;
+        s = s * zn_inv;
+    }
+    const uint32_t blocks = stream_blocks(ctx, n);
+    ProfScope ps_(ctx, PROF_POLY);
+    switch (logj) {
+        case 1: parts_idft_kernel<1><<<blocks, 256, 0, ctx->stream>>>(P, n); break;
+        case 2: parts_idft_kernel<2><<<blocks, 256, 0, ctx->stream>>>(P, n); break;
+        case 3: parts_idft_kernel<3><<<blocks, 256, 0, ctx->stream>>>(P, n); break;
+        case 4: parts_idft_kernel<4><<<blocks, 256, 0, ctx->stream>>>(P, n); break;
+        default: return fail(ctx, B200ZK_E_UNSUPPORTED, "parts_idft: J = 2^%u parts (2 <= J <= 16)", logj);
+    }
+    B2_LAUNCH_CHECK(ctx);
+    return B200ZK_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ linear combination
 // out[i] = sum_j s_j * p_j[i]: every input is read once and the output written once (a chain of axpy calls would move
 // 3x the bytes).  The SHPLONK prover's  sum_i v^i p_i(X)  per rotation set, and the final L(X) combination.
@@ -595,12 +674,17 @@ int32_t b200zk_graph_evaluate(b200zk_ctx* ctx, const b200zk_graph* graph, const 
                                       log_size <= 30 ? (1ull << log_size) : 0);
 }
 
-int32_t b200zk_graph_evaluate_rows(b200zk_ctx* ctx, const b200zk_graph* graph, const void* const* fixed_dev, uint32_t n_fixed,
-                                   const void* const* advice_dev, uint32_t n_advice, const void* const* instance_dev, uint32_t n_instance,
-                                   const void* challenges32, uint32_t n_challenges, const void* beta32, const void* gamma32,
-                                   const void* theta32, const void* y32, const void* extended_omega32, void* values_dev, uint32_t log_size,
-                                   int32_t rot_scale, uint64_t row_first, uint64_t row_count) {
-    CHECK_CTX(ctx);
+}  // extern "C"
+
+// part_log_N == 0: the whole extended domain of 2^log_size points, ExtendedX = zeta * extended_omega^row.
+// part_log_N > log_size: coset part `part` of the 2^part_log_N-point extended coset, evaluated as a domain of 2^log_size rows
+// with w = extended_omega^J, ExtendedX = (zeta * extended_omega^part) * w^row.
+static int32_t graph_evaluate_common(b200zk_ctx* ctx, const b200zk_graph* graph, const void* const* fixed_dev, uint32_t n_fixed,
+                                     const void* const* advice_dev, uint32_t n_advice, const void* const* instance_dev,
+                                     uint32_t n_instance, const void* challenges32, uint32_t n_challenges, const void* beta32,
+                                     const void* gamma32, const void* theta32, const void* y32, const void* extended_omega32,
+                                     void* values_dev, uint32_t log_size, int32_t rot_scale, uint64_t row_first, uint64_t row_count,
+                                     uint32_t part_log_N, uint32_t part) {
     if (!graph) return fail(ctx, B200ZK_E_INVALID, "graph_evaluate: null graph");
     if (log_size > 30) return fail(ctx, B200ZK_E_INVALID, "graph_evaluate: log_size = %u > 30", log_size);
     if (row_first > (1ull << log_size) || row_count > (1ull << log_size) - row_first)
@@ -652,12 +736,18 @@ int32_t b200zk_graph_evaluate_rows(b200zk_ctx* ctx, const b200zk_graph* graph, c
     L.zeta = host_zeta();
     L.row_first = row_first;
     L.row_count = row_count;
-    if (P.uses_x && log_size) {
+    if (P.uses_x && (log_size || part_log_N)) {
         Fr w;
         B2_TRY(read_fr(ctx, extended_omega32, &w));
-        const Fr* tab = nullptr;
-        B2_TRY(ntt_get_table(ctx, w, log_size, &tab));
-        L.xtab = tab + (size >> 1);
+        if (part_log_N) {  // x0 = zeta * extended_omega^part, w = extended_omega^J
+            L.zeta = L.zeta * w.pow_u64(part);
+            for (uint32_t i = log_size; i < part_log_N; ++i) w = w.sqr();
+        }
+        if (log_size) {
+            const Fr* tab = nullptr;
+            B2_TRY(ntt_get_table(ctx, w, log_size, &tab));
+            L.xtab = tab + (size >> 1);
+        }
     }
     // the small per-call tables ride on the context stream ahead of the kernel; a previous evaluate of this graph on
     // the same stream has finished reading them by then (stream order)
@@ -665,6 +755,31 @@ int32_t b200zk_graph_evaluate_rows(b200zk_ctx* ctx, const b200zk_graph* graph, c
     if (P.n_rotations) B2_CUDA(ctx, cudaMemcpyAsync(graph->dev_rot, rot_off.data(), sizeof(uint32_t) * P.n_rotations, cudaMemcpyHostToDevice, ctx->stream));
     if (graph->cols_cap) B2_CUDA(ctx, cudaMemcpyAsync(graph->dev_cols, cols.data(), sizeof(void*) * graph->cols_cap, cudaMemcpyHostToDevice, ctx->stream));
     return graph_evaluate_run(ctx, graph, L);
+}
+
+extern "C" {
+
+int32_t b200zk_graph_evaluate_rows(b200zk_ctx* ctx, const b200zk_graph* graph, const void* const* fixed_dev, uint32_t n_fixed,
+                                   const void* const* advice_dev, uint32_t n_advice, const void* const* instance_dev, uint32_t n_instance,
+                                   const void* challenges32, uint32_t n_challenges, const void* beta32, const void* gamma32,
+                                   const void* theta32, const void* y32, const void* extended_omega32, void* values_dev, uint32_t log_size,
+                                   int32_t rot_scale, uint64_t row_first, uint64_t row_count) {
+    CHECK_CTX(ctx);
+    return graph_evaluate_common(ctx, graph, fixed_dev, n_fixed, advice_dev, n_advice, instance_dev, n_instance, challenges32,
+                                 n_challenges, beta32, gamma32, theta32, y32, extended_omega32, values_dev, log_size, rot_scale,
+                                 row_first, row_count, 0, 0);
+}
+
+int32_t b200zk_graph_evaluate_part(b200zk_ctx* ctx, const b200zk_graph* graph, const void* const* fixed_dev, uint32_t n_fixed,
+                                   const void* const* advice_dev, uint32_t n_advice, const void* const* instance_dev, uint32_t n_instance,
+                                   const void* challenges32, uint32_t n_challenges, const void* beta32, const void* gamma32,
+                                   const void* theta32, const void* y32, const void* extended_omega32, void* values_dev, uint32_t k,
+                                   uint32_t extended_k, uint32_t part) {
+    CHECK_CTX(ctx);
+    B2_TRY(check_part(ctx, k, extended_k, part, "graph_evaluate_part"));
+    return graph_evaluate_common(ctx, graph, fixed_dev, n_fixed, advice_dev, n_advice, instance_dev, n_instance, challenges32,
+                                 n_challenges, beta32, gamma32, theta32, y32, extended_omega32, values_dev, k, 1, 0, 1ull << k,
+                                 extended_k, part);
 }
 
 }  // extern "C"

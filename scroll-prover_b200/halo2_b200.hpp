@@ -185,6 +185,30 @@ class EvaluationDomain {
         a.resize((size_t)(n * quotient_poly_degree));  // truncate to the quotient degree
         return a;
     }
+    // Coset parts: J = 2^(extended_k - k); part j of the extended coset is zeta * extended_omega^j * <omega>, i.e. extended
+    // rows j, j + J, j + 2J, ...  coeff_to_extended_part(a, j)[r] == coeff_to_extended(a)[j + J*r].
+    uint32_t n_parts() const { return 1u << (extended_k - k); }
+    std::vector<Fr> coeff_to_extended_part(const std::vector<Fr>& a, uint32_t part) const {
+        if (a.size() != n) throw Panic("assertion failed: a.values.len() == 1 << self.k");
+        std::vector<Fr> out(n);
+        auto& b = Backend::get();
+        b.check(b200zk_coeff_to_extended_part(b.ctx(), a.data(), k, extended_k, &extended_omega, part, out.data()), "coeff_to_extended_part");
+        return out;
+    }
+    // parts[j] = values on part j -> parts[t] = coefficients [t*n, (t+1)*n) of extended_to_coeff (before its truncation) of
+    // the interleaved coset, divided by X^n - 1 first when divide_by_vanishing
+    std::vector<std::vector<Fr>> extended_parts_to_coeff(std::vector<std::vector<Fr>> parts, bool divide_by_vanishing) const {
+        if (parts.size() != n_parts()) throw Panic("extended_parts_to_coeff: one vector per part");
+        std::vector<void*> ptrs;
+        for (auto& p : parts) {
+            if (p.size() != n) throw Panic("extended_parts_to_coeff: part length");
+            ptrs.push_back(p.data());
+        }
+        auto& b = Backend::get();
+        b.check(b200zk_extended_parts_to_coeff(b.ctx(), ptrs.data(), k, extended_k, &extended_omega, divide_by_vanishing ? 1 : 0),
+                "extended_parts_to_coeff");
+        return parts;
+    }
 };
 
 // halo2_proofs::poly::kzg::commitment::ParamsKZG<Bn256>

@@ -551,6 +551,50 @@ struct Ops {
     // mv_lookup phi(X) running sum
     virtual Poly logup_running_sum(const std::vector<const Poly*>& inputs, const Poly& table, const Poly& m, const Fr& beta,
                                    const Fr& phi_init) = 0;
+
+    // Coset parts of the extended domain: J = 2^(extended_k - k) parts of n rows, part j = extended rows j, j + J, j + 2J, ...
+    // The defaults are the whole-coset operations above, so a backend without part kernels computes the same values.
+    // coeff_to_extended_part(c, j)[r] == coeff_to_extended(c)[j + J*r]
+    virtual Poly coeff_to_extended_part(const Poly& coeffs, uint32_t part) {
+        const Poly ext = coeff_to_extended(coeffs);
+        const size_t n = coeffs.size(), J = ext.size() / n;
+        Poly out(n);
+        for (size_t r = 0; r < n; ++r) out[r] = ext[part + J * r];
+        return out;
+    }
+    // parts[j] = values on part j -> pieces of n coefficients (piece t = coefficients [t*n, (t+1)*n)) of extended_to_coeff of the
+    // interleaved coset, divided by X^n - 1 first when asked; at least the quotient_poly_degree pieces extended_to_coeff keeps
+    virtual std::vector<Poly> extended_parts_to_coeff(std::vector<Poly> parts, bool divide_by_vanishing) {
+        const size_t J = parts.size(), n = parts[0].size();
+        Poly ext(J * n);
+        for (size_t j = 0; j < J; ++j)
+            for (size_t r = 0; r < n; ++r) ext[j + J * r] = parts[j][r];
+        if (divide_by_vanishing) {  // (zeta * w_ext^j)^n - 1 on part j
+            uint32_t ext_k = 0;
+            while (((size_t)1 << ext_k) < J * n) ++ext_k;
+            DFr eo = detail::root_of_unity();
+            for (uint32_t i = ext_k; i < 28; ++i) eo = eo.sqr();
+            const Fr wn = f_pow(from_dev(eo), n);
+            Fr cur = f_pow(from_dev(detail::zeta()), n);
+            std::vector<Fr> t_inv(J);
+            for (auto& t : t_inv) { t = f_inv(f_sub(cur, f_one())); cur = f_mul(cur, wn); }
+            Poly t_col(J * n);
+            for (size_t i = 0; i < J * n; ++i) t_col[i] = t_inv[i % J];
+            ext = poly_mul(ext, t_col);
+        }
+        const Poly c = extended_to_coeff(std::move(ext));
+        std::vector<Poly> pieces;
+        for (size_t t = 0; (t + 1) * n <= c.size(); ++t) pieces.emplace_back(c.begin() + t * n, c.begin() + (t + 1) * n);
+        return pieces;
+    }
+    // graph_evaluate on part `part`: every column and values hold the n values of that part
+    virtual void graph_evaluate_part(const Program& p, const std::vector<const Poly*>& fixed, const std::vector<const Poly*>& advice,
+                                     const std::vector<const Poly*>& instance, const std::vector<Fr>& challenges, const Fr& beta,
+                                     const Fr& gamma, const Fr& theta, const Fr& y, uint32_t part, Poly& values) {
+        (void)p, (void)fixed, (void)advice, (void)instance, (void)challenges, (void)beta, (void)gamma, (void)theta, (void)y, (void)part,
+            (void)values;
+        throw Panic("graph_evaluate_part: this backend evaluates whole cosets only");
+    }
 };
 
 // The product: every operation through the C ABI.  Host vectors in and out (the ABI stages them); the quotient-construction
@@ -591,29 +635,16 @@ class DeviceOps : public Ops {
     void graph_evaluate(const Program& p, const std::vector<const Poly*>& fixed, const std::vector<const Poly*>& advice,
                         const std::vector<const Poly*>& instance, const std::vector<Fr>& challenges, const Fr& beta, const Fr& gamma,
                         const Fr& theta, const Fr& y, Poly& values) override {
-        auto& be = Backend::get();
-        b200zk_graph* g = nullptr;
-        be.check(b200zk_graph_create(be.ctx(), p.calcs.data(), (uint32_t)p.calcs.size(), p.parts.data(), (uint32_t)p.parts.size(),
-                                     p.constants.data(), (uint32_t)p.constants.size(), p.rotations.data(), (uint32_t)p.rotations.size(), &g),
-                 "graph_create");
-        std::vector<DeviceColumn> keep;
-        auto up = [&](const std::vector<const Poly*>& v) {
-            std::vector<const void*> t;
-            for (auto* c : v) {
-                keep.emplace_back(*c);
-                t.push_back(keep.back().ptr());
-            }
-            return t;
-        };
-        keep.reserve(fixed.size() + advice.size() + instance.size() + 1);
-        auto tf = up(fixed), ta = up(advice), ti = up(instance);
-        DeviceColumn vals(values);
-        int32_t rc = b200zk_graph_evaluate(be.ctx(), g, tf.data(), (uint32_t)tf.size(), ta.data(), (uint32_t)ta.size(), ti.data(),
-                                           (uint32_t)ti.size(), challenges.data(), (uint32_t)challenges.size(), &beta, &gamma, &theta, &y,
-                                           &dom_.extended_omega, vals.ptr(), dom_.extended_k, 1 << (dom_.extended_k - dom_.k));
-        b200zk_graph_destroy(be.ctx(), g);
-        be.check(rc, "graph_evaluate");
-        values = vals.to_host();
+        run_graph(p, fixed, advice, instance, challenges, beta, gamma, theta, y, -1, values);
+    }
+    Poly coeff_to_extended_part(const Poly& c, uint32_t part) override { return dom_.coeff_to_extended_part(c, part); }
+    std::vector<Poly> extended_parts_to_coeff(std::vector<Poly> parts, bool divide_by_vanishing) override {
+        return dom_.extended_parts_to_coeff(std::move(parts), divide_by_vanishing);
+    }
+    void graph_evaluate_part(const Program& p, const std::vector<const Poly*>& fixed, const std::vector<const Poly*>& advice,
+                             const std::vector<const Poly*>& instance, const std::vector<Fr>& challenges, const Fr& beta, const Fr& gamma,
+                             const Fr& theta, const Fr& y, uint32_t part, Poly& values) override {
+        run_graph(p, fixed, advice, instance, challenges, beta, gamma, theta, y, (int64_t)part, values);
     }
     Poly permutation_product(const std::vector<const Poly*>& values, const std::vector<const Poly*>& sigma, const Fr& beta, const Fr& gamma,
                              const Fr& delta_omega_start, const Fr& delta, const Fr& z_init) override {
@@ -637,6 +668,40 @@ class DeviceOps : public Ops {
     }
 
   private:
+    // part < 0: the whole extended coset (b200zk_graph_evaluate); else that coset part (b200zk_graph_evaluate_part)
+    void run_graph(const Program& p, const std::vector<const Poly*>& fixed, const std::vector<const Poly*>& advice,
+                   const std::vector<const Poly*>& instance, const std::vector<Fr>& challenges, const Fr& beta, const Fr& gamma,
+                   const Fr& theta, const Fr& y, int64_t part, Poly& values) {
+        auto& be = Backend::get();
+        b200zk_graph* g = nullptr;
+        be.check(b200zk_graph_create(be.ctx(), p.calcs.data(), (uint32_t)p.calcs.size(), p.parts.data(), (uint32_t)p.parts.size(),
+                                     p.constants.data(), (uint32_t)p.constants.size(), p.rotations.data(), (uint32_t)p.rotations.size(), &g),
+                 "graph_create");
+        std::vector<DeviceColumn> keep;
+        auto up = [&](const std::vector<const Poly*>& v) {
+            std::vector<const void*> t;
+            for (auto* c : v) {
+                keep.emplace_back(*c);
+                t.push_back(keep.back().ptr());
+            }
+            return t;
+        };
+        keep.reserve(fixed.size() + advice.size() + instance.size() + 1);
+        auto tf = up(fixed), ta = up(advice), ti = up(instance);
+        DeviceColumn vals(values);
+        int32_t rc = part < 0
+                         ? b200zk_graph_evaluate(be.ctx(), g, tf.data(), (uint32_t)tf.size(), ta.data(), (uint32_t)ta.size(), ti.data(),
+                                                 (uint32_t)ti.size(), challenges.data(), (uint32_t)challenges.size(), &beta, &gamma, &theta,
+                                                 &y, &dom_.extended_omega, vals.ptr(), dom_.extended_k, 1 << (dom_.extended_k - dom_.k))
+                         : b200zk_graph_evaluate_part(be.ctx(), g, tf.data(), (uint32_t)tf.size(), ta.data(), (uint32_t)ta.size(),
+                                                      ti.data(), (uint32_t)ti.size(), challenges.data(), (uint32_t)challenges.size(), &beta,
+                                                      &gamma, &theta, &y, &dom_.extended_omega, vals.ptr(), dom_.k, dom_.extended_k,
+                                                      (uint32_t)part);
+        b200zk_graph_destroy(be.ctx(), g);
+        be.check(rc, part < 0 ? "graph_evaluate" : "graph_evaluate_part");
+        values = vals.to_host();
+    }
+
     ParamsKZG& params_;
     const EvaluationDomain& dom_;
 };
@@ -669,9 +734,11 @@ struct VerifyingKey {
 };
 struct ProvingKey {
     VerifyingKey vk;
-    Poly l0, l_last, l_active_row;                       // extended cosets
+    Poly l0, l_last, l_active_row;                       // extended cosets (empty in a key without cosets)
     std::vector<Poly> fixed_values, fixed_polys, fixed_cosets;
     std::vector<Poly> sigma_values, sigma_polys, sigma_cosets;
+    Poly l0_poly, l_last_poly, l_blind_poly;              // coefficient forms, kept instead of the cosets (keygen keep_cosets = false)
+    bool has_cosets() const { return !l0.empty(); }
     Program gates;                                        // custom gates folded with y
     Program permutation;                                  // evaluate_h "Permutations" section
     std::vector<Program> lookups;                         // one program per lookup
@@ -718,8 +785,11 @@ inline AuxLayout aux_layout(const ConstraintSystem& cs) {
     return a;
 }
 
-// keygen_vk + keygen_pk: fixed columns (Lagrange values), the permutation assembly; polynomials and cosets through `ops`
-inline ProvingKey keygen(Ops& ops, const EvaluationDomain& dom, ConstraintSystem cs, const std::vector<Poly>& fixed, const Assembly& assembly) {
+// keygen_vk + keygen_pk: fixed columns (Lagrange values), the permutation assembly; polynomials and cosets through `ops`.
+// keep_cosets = false: the key stores no extended coset (J*n values per fixed / permutation column and l0 / l_last /
+// l_active_row), only the coefficient forms; create_proof then computes evaluate_h one coset part at a time.
+inline ProvingKey keygen(Ops& ops, const EvaluationDomain& dom, ConstraintSystem cs, const std::vector<Poly>& fixed, const Assembly& assembly,
+                         bool keep_cosets = true) {
     if (cs.advice_queries.empty() && cs.fixed_queries.empty()) cs.finalize();
     const uint64_t n = dom.n;
     if (fixed.size() != cs.num_fixed) throw Panic("keygen: wrong number of fixed columns");
@@ -745,7 +815,7 @@ inline ProvingKey keygen(Ops& ops, const EvaluationDomain& dom, ConstraintSystem
         pk.fixed_values.push_back(col);
         pk.vk.fixed_commitments.push_back(to_affine_point(ops.commit_lagrange(col)));
         pk.fixed_polys.push_back(ops.lagrange_to_coeff(col));
-        pk.fixed_cosets.push_back(ops.coeff_to_extended(pk.fixed_polys.back()));
+        if (keep_cosets) pk.fixed_cosets.push_back(ops.coeff_to_extended(pk.fixed_polys.back()));
     }
     // permutation::keygen::Assembly::build_{vk,pk}: sigma_i(omega^j) = delta^{i'} omega^{j'} for mapping[i][j] = (i', j')
     const Fr delta = f_delta();
@@ -763,7 +833,7 @@ inline ProvingKey keygen(Ops& ops, const EvaluationDomain& dom, ConstraintSystem
         pk.sigma_values.push_back(s);
         pk.vk.permutation_commitments.push_back(to_affine_point(ops.commit_lagrange(s)));
         pk.sigma_polys.push_back(ops.lagrange_to_coeff(s));
-        pk.sigma_cosets.push_back(ops.coeff_to_extended(pk.sigma_polys.back()));
+        if (keep_cosets) pk.sigma_cosets.push_back(ops.coeff_to_extended(pk.sigma_polys.back()));
     }
     // l0, l_last, l_active_row (keygen_pk): l_blind covers the last blinding_factors rows, l_last the row before them
     const uint32_t bf = cs.blinding_factors();
@@ -772,11 +842,17 @@ inline ProvingKey keygen(Ops& ops, const EvaluationDomain& dom, ConstraintSystem
     l0[0] = f_one();
     for (uint64_t r = n - bf; r < n; ++r) l_blind[r] = f_one();
     l_last[n - bf - 1] = f_one();
-    pk.l0 = ops.coeff_to_extended(ops.lagrange_to_coeff(l0));
-    Poly lb = ops.coeff_to_extended(ops.lagrange_to_coeff(l_blind));
-    pk.l_last = ops.coeff_to_extended(ops.lagrange_to_coeff(l_last));
-    pk.l_active_row.resize(pk.l0.size());
-    for (size_t i = 0; i < pk.l0.size(); ++i) pk.l_active_row[i] = f_sub(f_sub(f_one(), pk.l_last[i]), lb[i]);
+    if (keep_cosets) {
+        pk.l0 = ops.coeff_to_extended(ops.lagrange_to_coeff(l0));
+        Poly lb = ops.coeff_to_extended(ops.lagrange_to_coeff(l_blind));
+        pk.l_last = ops.coeff_to_extended(ops.lagrange_to_coeff(l_last));
+        pk.l_active_row.resize(pk.l0.size());
+        for (size_t i = 0; i < pk.l0.size(); ++i) pk.l_active_row[i] = f_sub(f_sub(f_one(), pk.l_last[i]), lb[i]);
+    } else {
+        pk.l0_poly = ops.lagrange_to_coeff(l0);
+        pk.l_blind_poly = ops.lagrange_to_coeff(l_blind);
+        pk.l_last_poly = ops.lagrange_to_coeff(l_last);
+    }
     pk.vk.transcript_repr = vk_transcript_repr(pk.vk);
 
     // ---- Evaluator::new: the programs of evaluate_h
@@ -951,6 +1027,7 @@ inline ProofArtifacts create_proof(Ops& ops, const EvaluationDomain& dom, const 
     const uint32_t bf = cs.blinding_factors();
     const uint64_t u = n - bf - 1;  // last usable row index (the l_last row); rows > u are blinding rows
     const AuxLayout aux = aux_layout(cs);
+    const bool by_parts = !pk.has_cosets();  // evaluate_h one coset part at a time, from coefficient forms
     if (instances.size() != cs.num_instance) throw Panic("create_proof: wrong number of columns");
     if (!cs.advice_phase.empty() && cs.advice_phase.size() != cs.num_advice) throw Panic("create_proof: one phase per advice column");
     Rng rng(rng_seed);
@@ -966,7 +1043,7 @@ inline ProofArtifacts create_proof(Ops& ops, const EvaluationDomain& dom, const 
         for (uint64_t r = u; r < n; ++r)
             if (!f_is_zero(inst[r])) throw Panic("create_proof: instance values beyond the usable rows");
         instance_polys.push_back(ops.lagrange_to_coeff(inst));
-        instance_cosets.push_back(ops.coeff_to_extended(instance_polys.back()));
+        if (!by_parts) instance_cosets.push_back(ops.coeff_to_extended(instance_polys.back()));
     }
     for (auto& inst : instances)
         for (uint64_t r = 0; r < u; ++r) tr.common_scalar(inst[r]);
@@ -992,7 +1069,7 @@ inline ProofArtifacts create_proof(Ops& ops, const EvaluationDomain& dom, const 
     }
     for (auto& col : advice) {
         advice_polys.push_back(ops.lagrange_to_coeff(col));
-        advice_cosets.push_back(ops.coeff_to_extended(advice_polys.back()));
+        if (!by_parts) advice_cosets.push_back(ops.coeff_to_extended(advice_polys.back()));
     }
     const Fr theta = tr.squeeze_challenge();
 
@@ -1063,7 +1140,7 @@ inline ProofArtifacts create_proof(Ops& ops, const EvaluationDomain& dom, const 
         for (auto& z : z_values) write_point(ops.commit_lagrange(z));
         for (auto& z : z_values) {
             z_polys.push_back(ops.lagrange_to_coeff(z));
-            z_cosets.push_back(ops.coeff_to_extended(z_polys.back()));
+            if (!by_parts) z_cosets.push_back(ops.coeff_to_extended(z_polys.back()));
         }
     }
     // 4. lookups, second half (commit_grand_sum): phi running sum, blinded, committed
@@ -1080,42 +1157,83 @@ inline ProofArtifacts create_proof(Ops& ops, const EvaluationDomain& dom, const 
     const Fr y = tr.squeeze_challenge();
 
     // 6. evaluate_h on the extended coset: gates, permutation, lookups folded with y; divide by X^n - 1
-    const size_t ext_n = (size_t)1 << dom.extended_k;
-    Poly h_ext(ext_n, f_zero());
-    std::vector<const Poly*> fixed_tab, advice_tab, instance_tab;
-    for (auto& c : pk.fixed_cosets) fixed_tab.push_back(&c);
-    fixed_tab.push_back(&pk.l0);
-    fixed_tab.push_back(&pk.l_last);
-    fixed_tab.push_back(&pk.l_active_row);
-    for (auto& c : pk.sigma_cosets) fixed_tab.push_back(&c);
-    for (auto& c : advice_cosets) advice_tab.push_back(&c);
-    for (auto& c : z_cosets) advice_tab.push_back(&c);
-    std::vector<Poly> lk_cosets;  // m, phi cosets per lookup
-    lk_cosets.reserve(2 * lk.size());
     for (auto& l : lk) {
         l.m_poly = ops.lagrange_to_coeff(l.m);
         l.phi_poly = ops.lagrange_to_coeff(l.phi);
-        lk_cosets.push_back(ops.coeff_to_extended(l.m_poly));
-        lk_cosets.push_back(ops.coeff_to_extended(l.phi_poly));
     }
-    for (auto& c : lk_cosets) advice_tab.push_back(&c);
-    for (auto& c : instance_cosets) instance_tab.push_back(&c);
-    if (!pk.gates.calcs.empty()) ops.graph_evaluate(pk.gates, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, h_ext);
-    if (!cs.permutation.empty()) ops.graph_evaluate(pk.permutation, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, h_ext);
-    for (auto& prog : pk.lookups) ops.graph_evaluate(prog, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, h_ext);
-    {   // EvaluationDomain::divide_by_vanishing_poly: (zeta * w_ext^i)^n - 1 takes 2^(extended_k - k) distinct values
-        const size_t period = (size_t)1 << (dom.extended_k - dom.k);
-        std::vector<Fr> t_inv(period);
-        Fr zn = f_pow(dom.g_coset, n), wn = f_pow(dom.extended_omega, n), cur = zn;
-        for (size_t i = 0; i < period; ++i) { t_inv[i] = f_inv(f_sub(cur, f_one())); cur = f_mul(cur, wn); }
-        Poly t_col(ext_n);
-        for (size_t i = 0; i < ext_n; ++i) t_col[i] = t_inv[i % period];
-        h_ext = ops.poly_mul(h_ext, t_col);
+    std::vector<Poly> h_pieces;  // vanishing::Committed::construct: pieces of n coefficients, each committed
+    if (!by_parts) {
+        const size_t ext_n = (size_t)1 << dom.extended_k;
+        Poly h_ext(ext_n, f_zero());
+        std::vector<const Poly*> fixed_tab, advice_tab, instance_tab;
+        for (auto& c : pk.fixed_cosets) fixed_tab.push_back(&c);
+        fixed_tab.push_back(&pk.l0);
+        fixed_tab.push_back(&pk.l_last);
+        fixed_tab.push_back(&pk.l_active_row);
+        for (auto& c : pk.sigma_cosets) fixed_tab.push_back(&c);
+        for (auto& c : advice_cosets) advice_tab.push_back(&c);
+        for (auto& c : z_cosets) advice_tab.push_back(&c);
+        std::vector<Poly> lk_cosets;  // m, phi cosets per lookup
+        lk_cosets.reserve(2 * lk.size());
+        for (auto& l : lk) {
+            lk_cosets.push_back(ops.coeff_to_extended(l.m_poly));
+            lk_cosets.push_back(ops.coeff_to_extended(l.phi_poly));
+        }
+        for (auto& c : lk_cosets) advice_tab.push_back(&c);
+        for (auto& c : instance_cosets) instance_tab.push_back(&c);
+        if (!pk.gates.calcs.empty()) ops.graph_evaluate(pk.gates, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, h_ext);
+        if (!cs.permutation.empty()) ops.graph_evaluate(pk.permutation, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, h_ext);
+        for (auto& prog : pk.lookups) ops.graph_evaluate(prog, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, h_ext);
+        {   // EvaluationDomain::divide_by_vanishing_poly: (zeta * w_ext^i)^n - 1 takes 2^(extended_k - k) distinct values
+            const size_t period = (size_t)1 << (dom.extended_k - dom.k);
+            std::vector<Fr> t_inv(period);
+            Fr zn = f_pow(dom.g_coset, n), wn = f_pow(dom.extended_omega, n), cur = zn;
+            for (size_t i = 0; i < period; ++i) { t_inv[i] = f_inv(f_sub(cur, f_one())); cur = f_mul(cur, wn); }
+            Poly t_col(ext_n);
+            for (size_t i = 0; i < ext_n; ++i) t_col[i] = t_inv[i % period];
+            h_ext = ops.poly_mul(h_ext, t_col);
+        }
+        Poly h_coeffs = ops.extended_to_coeff(std::move(h_ext));  // n * quotient_poly_degree coefficients
+        for (size_t i = 0; i < dom.quotient_poly_degree; ++i) h_pieces.emplace_back(h_coeffs.begin() + i * n, h_coeffs.begin() + (i + 1) * n);
+    } else {
+        // by coset parts: per part j, every column's n values on zeta * w_ext^j * <omega> from its coefficients, the same
+        // programs with rotations inside the part, then the J parts back to coefficients with the division by X^n - 1.
+        // Column tables as above: fixed = [fixed..., l0, l_last, l_active, sigma...], advice = [advice..., z..., m/phi...].
+        std::vector<const Poly*> fixed_c, advice_c, instance_c;
+        for (auto& c : pk.fixed_polys) fixed_c.push_back(&c);
+        fixed_c.push_back(&pk.l0_poly);
+        fixed_c.push_back(&pk.l_last_poly);
+        fixed_c.push_back(&pk.l_blind_poly);  // its part becomes l_active_row = 1 - l_last - l_blind, pointwise
+        for (auto& c : pk.sigma_polys) fixed_c.push_back(&c);
+        for (auto& c : advice_polys) advice_c.push_back(&c);
+        for (auto& c : z_polys) advice_c.push_back(&c);
+        for (auto& l : lk) { advice_c.push_back(&l.m_poly); advice_c.push_back(&l.phi_poly); }
+        for (auto& c : instance_polys) instance_c.push_back(&c);
+        const uint32_t J = 1u << (dom.extended_k - dom.k), l_active = aux.l_active;
+        std::vector<Poly> h_parts(J);
+        for (uint32_t j = 0; j < J; ++j) {
+            auto parts_of = [&](const std::vector<const Poly*>& cs_) {
+                std::vector<Poly> out;
+                out.reserve(cs_.size());
+                for (auto* c : cs_) out.push_back(ops.coeff_to_extended_part(*c, j));
+                return out;
+            };
+            std::vector<Poly> fp = parts_of(fixed_c), ap = parts_of(advice_c), ip = parts_of(instance_c);
+            for (uint64_t r = 0; r < n; ++r) fp[l_active][r] = f_sub(f_sub(f_one(), fp[l_active - 1][r]), fp[l_active][r]);
+            std::vector<const Poly*> fixed_tab, advice_tab, instance_tab;
+            for (auto& c : fp) fixed_tab.push_back(&c);
+            for (auto& c : ap) advice_tab.push_back(&c);
+            for (auto& c : ip) instance_tab.push_back(&c);
+            Poly& v = h_parts[j];
+            v.assign(n, f_zero());
+            if (!pk.gates.calcs.empty()) ops.graph_evaluate_part(pk.gates, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, j, v);
+            if (!cs.permutation.empty()) ops.graph_evaluate_part(pk.permutation, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, j, v);
+            for (auto& prog : pk.lookups) ops.graph_evaluate_part(prog, fixed_tab, advice_tab, instance_tab, challenges, beta, gamma, theta, y, j, v);
+        }
+        h_pieces = ops.extended_parts_to_coeff(std::move(h_parts), true);
+        if (h_pieces.size() < dom.quotient_poly_degree) throw Panic("create_proof: extended_parts_to_coeff returned too few pieces");
+        h_pieces.resize(dom.quotient_poly_degree);
     }
-    Poly h_coeffs = ops.extended_to_coeff(std::move(h_ext));  // n * quotient_poly_degree coefficients
-    // vanishing::Committed::construct: pieces of n coefficients, each committed
-    std::vector<Poly> h_pieces;
-    for (size_t i = 0; i < dom.quotient_poly_degree; ++i) h_pieces.emplace_back(h_coeffs.begin() + i * n, h_coeffs.begin() + (i + 1) * n);
     for (auto& p : h_pieces) write_point(ops.commit(p));
     const Fr x = tr.squeeze_challenge();
     const Fr xn = f_pow(x, n);
