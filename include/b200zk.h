@@ -253,6 +253,17 @@ B200ZK_API int32_t b200zk_logup_running_sum(b200zk_ctx* ctx, const void* const* 
                                             const void* table_dev, const void* m_dev, const void* beta32, uint32_t k,
                                             const void* phi_init32, void* phi_out_dev);
 
+/* mv_lookup::Argument::prepare, the m(X) column: for every input column j < n_inputs and row i < usable, the table
+ * row t < usable holding the same value gets one count, t = the FIRST such row; m_out_dev[t] = count (Montgomery Fr),
+ * every other row (and every row >= usable) zero.  Values are compared as canonical limbs.  *first_missing (host) =
+ * j * 2^k + i of the smallest (j, i) whose value is in no usable table row, UINT64_MAX when none (m_out is then
+ * unspecified); that is a witness property, not an error, so the status is still B200ZK_OK.
+ * inputs_dev: n_inputs device columns, table_dev and m_out_dev: device columns of 2^k elements.
+ * 1 <= n_inputs <= 64, k <= 28, usable <= 2^k; anything else, or a host column, is B200ZK_E_INVALID. */
+B200ZK_API int32_t b200zk_lookup_multiplicities(b200zk_ctx* ctx, const void* const* inputs_dev, uint32_t n_inputs,
+                                                const void* table_dev, uint32_t k, uint64_t usable, void* m_out_dev,
+                                                uint64_t* first_missing);
+
 /* plonk::evaluation::GraphEvaluator on the device.  A program is the upstream `calculations` list: calculation i
  * writes intermediate i; operands are ValueSources.  Calculation::Horner(start, parts, factor) names its parts as a
  * range of `horner_parts`.  B200ZK_SRC_EXTENDED_X is an addition over upstream: the point zeta * extended_omega^row of

@@ -112,6 +112,21 @@ pub(crate) fn graph_evaluate_part(graph: *const sys::Graph, fixed_dev: &[*const 
     });
 }
 
+/// mv_lookup::Argument::prepare, the multiplicity column: m_dev[t] = how many (input, row < usable) cells hold the value of
+/// table row t, counted on the first usable row with that value.  All columns are device memory of 2^k elements.  A value in
+/// no usable table row is the error prepare returns for it (ConstraintSystemFailure), not a panic.
+pub(crate) fn lookup_multiplicities(inputs_dev: &[*const c_void], table_dev: *const c_void, k: u32, usable: u64,
+                                    m_dev: *mut c_void) -> Result<(), crate::plonk::Error> {
+    let mut first_missing = u64::MAX;
+    check(unsafe {
+        sys::b200zk_lookup_multiplicities(ctx(), inputs_dev.as_ptr(), inputs_dev.len() as u32, table_dev, k, usable, m_dev, &mut first_missing)
+    });
+    if first_missing != u64::MAX {
+        return Err(crate::plonk::Error::ConstraintSystemFailure);
+    }
+    Ok(())
+}
+
 pub(crate) fn eval_polynomial(poly: &[Fr], point: Fr) -> Fr {
     let mut out = Fr::zero();
     check(unsafe { sys::b200zk_eval_poly(ctx(), poly.as_ptr() as _, poly.len() as u64, p(&point), &mut out as *mut Fr as _) });

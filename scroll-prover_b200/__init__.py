@@ -100,6 +100,7 @@ def _signatures():
         "b200zk_poly_lincomb": [vp, vp, C.POINTER(vp), vp, u32, u64],
         "b200zk_permutation_product": [vp, C.POINTER(vp), C.POINTER(vp), u32, vp, vp, vp, vp, vp, u32, vp, vp],
         "b200zk_logup_running_sum": [vp, C.POINTER(vp), u32, vp, vp, vp, u32, vp, vp],
+        "b200zk_lookup_multiplicities": [vp, C.POINTER(vp), u32, vp, u32, u64, vp, C.POINTER(u64)],
         "b200zk_graph_create": [vp, vp, u32, vp, u32, vp, u32, vp, u32, C.POINTER(vp)],
         "b200zk_graph_check": [vp, u32, vp, u32, u32, u32, C.POINTER(u32), C.POINTER(u32), C.c_char_p, u64],
         "b200zk_graph_destroy": [vp, vp],
@@ -424,6 +425,17 @@ class Context:
         po, k5 = _ptr(out)
         self._ck(lib().b200zk_logup_running_sum(self._h, ti, len(inputs), pt, pm, pb, k, pp, po))
         return out
+
+    def lookup_multiplicities(self, inputs, table, k: int, usable: int, out):
+        """mv_lookup::Argument::prepare, the m(X) column, into `out` (device, 2^k elements): every (input j, row i < usable)
+        counts once on the first usable table row holding its value.  Returns None, or j * 2^k + i of the first cell whose
+        value is in no usable table row (the witness does not satisfy the lookup; `out` is then unspecified)."""
+        ti, ki = self._dev_table(inputs)
+        pt, k1 = _ptr(table)
+        po, k2 = _ptr(out)
+        missing = C.c_uint64()
+        self._ck(lib().b200zk_lookup_multiplicities(self._h, ti, len(inputs), pt, k, usable, po, C.byref(missing)))
+        return None if missing.value == (1 << 64) - 1 else missing.value
 
     def graph(self, calcs, constants, rotations) -> "Graph":
         return Graph(self, calcs, constants, rotations)

@@ -586,6 +586,20 @@ inline void logup_running_sum(const std::vector<const DeviceColumn*>& inputs, co
             "logup_running_sum");
 }
 
+// mv_lookup::Argument::prepare, the m(X) column: m_out[t] = the number of (input, row < usable) cells equal to table row t,
+// counted on the first usable table row holding that value.  Returns j * n + i of the first (input j, row i) whose value is
+// in no usable table row -- the witness does not satisfy the lookup, m_out is then unspecified -- or UINT64_MAX.
+inline uint64_t lookup_multiplicities(const std::vector<const DeviceColumn*>& inputs, const DeviceColumn& table, const EvaluationDomain& dom,
+                                      uint64_t usable, DeviceColumn& m_out) {
+    std::vector<const void*> ti;
+    for (auto* c : inputs) ti.push_back(c->ptr());
+    uint64_t first_missing = UINT64_MAX;
+    auto& b = Backend::get();
+    b.check(b200zk_lookup_multiplicities(b.ctx(), ti.data(), (uint32_t)ti.size(), table.ptr(), dom.k, usable, m_out.ptr(), &first_missing),
+            "lookup_multiplicities");
+    return first_missing;
+}
+
 }  // namespace plonk
 
 }  // namespace halo2_b200

@@ -11,10 +11,10 @@
 //
 // Every field-vector / group operation of the prover goes through the `Ops` interface below -- exactly the operations
 // libb200zk replaces (commit_lagrange, commit, lagrange_to_coeff, coeff_to_extended, extended_to_coeff, GraphEvaluator,
-// permutation product, log-derivative sum, eval_polynomial, kate_division, linear combinations).  `DeviceOps` implements it
+// permutation product, lookup multiplicities, log-derivative sum, eval_polynomial, kate_division, linear combinations).  `DeviceOps` implements it
 // over the C ABI (include/b200zk.h); the tests implement the same interface over the CPU oracle and require IDENTICAL PROOF
 // BYTES from both.  The host keeps what upstream keeps on the host: the transcript, challenge arithmetic, blinding rows,
-// multiplicity counting, rotation-set bookkeeping.  The verifier is host-only (pairing_bn254.hpp), as in the reference.
+// rotation-set bookkeeping.  The verifier is host-only (pairing_bn254.hpp), as in the reference.
 //
 // Fidelity: the phase loop (advice columns and challenges per phase, ConstraintSystem::{advice_column_phase, challenge_phase}),
 // argument order, constraint order, y-folding, evaluation order and the SHPLONK construction follow upstream;
@@ -551,6 +551,28 @@ struct Ops {
     // mv_lookup phi(X) running sum
     virtual Poly logup_running_sum(const std::vector<const Poly*>& inputs, const Poly& table, const Poly& m, const Fr& beta,
                                    const Fr& phi_init) = 0;
+    // mv_lookup::Argument::prepare, the m(X) column: every (input, row < usable) counts once on the FIRST usable table row
+    // holding its value; rows >= usable stay zero.  A value in no usable table row throws.  The default is the host index.
+    virtual Poly lookup_multiplicities(const std::vector<const Poly*>& inputs, const Poly& table, uint64_t usable) {
+        const size_t n = table.size();
+        std::map<std::array<uint64_t, 4>, uint64_t> index;  // table value -> first row holding it (usable rows only)
+        for (uint64_t r = 0; r < usable; ++r) {
+            std::array<uint64_t, 4> key{table[r].l[0], table[r].l[1], table[r].l[2], table[r].l[3]};
+            index.emplace(key, r);
+        }
+        std::vector<uint64_t> counts(n, 0);
+        for (const Poly* in : inputs)
+            for (uint64_t r = 0; r < usable; ++r) {
+                std::array<uint64_t, 4> key{(*in)[r].l[0], (*in)[r].l[1], (*in)[r].l[2], (*in)[r].l[3]};
+                auto it = index.find(key);
+                if (it == index.end()) throw Panic(lookup_missing_message());
+                counts[it->second]++;
+            }
+        Poly m(n);
+        for (size_t r = 0; r < n; ++r) m[r] = f_u64(counts[r]);
+        return m;
+    }
+    static const char* lookup_missing_message() { return "lookup input is not in the table (the witness does not satisfy the lookup)"; }
 
     // Coset parts of the extended domain: J = 2^(extended_k - k) parts of n rows, part j = extended rows j, j + J, j + 2J, ...
     // The defaults are the whole-coset operations above, so a backend without part kernels computes the same values.
@@ -665,6 +687,15 @@ class DeviceOps : public Ops {
         DeviceColumn t(table), mm(m), phi((size_t)dom_.n);
         plonk::logup_running_sum(di, t, mm, beta, dom_, phi_init, phi);
         return phi.to_host();
+    }
+    Poly lookup_multiplicities(const std::vector<const Poly*>& inputs, const Poly& table, uint64_t usable) override {
+        std::vector<DeviceColumn> keep;
+        keep.reserve(inputs.size());
+        std::vector<const DeviceColumn*> di;
+        for (auto* c : inputs) { keep.emplace_back(*c); di.push_back(&keep.back()); }
+        DeviceColumn t(table), m((size_t)dom_.n);
+        if (plonk::lookup_multiplicities(di, t, dom_, usable, m) != UINT64_MAX) throw Panic(lookup_missing_message());
+        return m.to_host();
     }
 
   private:
@@ -1098,20 +1129,7 @@ inline ProofArtifacts create_proof(Ops& ops, const EvaluationDomain& dom, const 
     for (size_t li = 0; li < cs.lookups.size(); ++li) {
         lk[li].input = compress(cs.lookups[li].inputs);
         lk[li].table = compress(cs.lookups[li].table);
-        lk[li].m.assign(n, f_zero());
-        std::map<std::array<uint64_t, 4>, uint64_t> index;  // table value -> first row holding it (usable rows only)
-        for (uint64_t r = 0; r < u; ++r) {
-            std::array<uint64_t, 4> key{lk[li].table[r].l[0], lk[li].table[r].l[1], lk[li].table[r].l[2], lk[li].table[r].l[3]};
-            index.emplace(key, r);
-        }
-        std::vector<uint64_t> counts(n, 0);
-        for (uint64_t r = 0; r < u; ++r) {
-            std::array<uint64_t, 4> key{lk[li].input[r].l[0], lk[li].input[r].l[1], lk[li].input[r].l[2], lk[li].input[r].l[3]};
-            auto it = index.find(key);
-            if (it == index.end()) throw Panic("lookup input is not in the table (the witness does not satisfy the lookup)");
-            counts[it->second]++;
-        }
-        for (uint64_t r = 0; r < n; ++r) lk[li].m[r] = f_u64(counts[r]);
+        lk[li].m = ops.lookup_multiplicities({&lk[li].input}, lk[li].table, u);
         write_point(ops.commit_lagrange(lk[li].m));
     }
     const Fr beta = tr.squeeze_challenge();
