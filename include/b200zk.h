@@ -310,10 +310,12 @@ B200ZK_API int32_t b200zk_graph_check(const b200zk_calculation* calculations, ui
                                       uint64_t message_cap);
 B200ZK_API int32_t b200zk_graph_destroy(b200zk_ctx* ctx, b200zk_graph* graph);
 B200ZK_API int32_t b200zk_graph_info(const b200zk_graph* graph, uint32_t* n_instructions, uint32_t* n_slots);
-/* GraphEvaluator::evaluate for every row of the extended domain: values[row] = result of the last calculation, with
+/* GraphEvaluator::evaluate for every row of a domain of 2^log_size rows: values[row] = result of the last calculation, with
  * PreviousValue = the old values[row] (so successive programs chain the way evaluate_h folds gates with y) and
- * column reads at (row + rotations[r] * rot_scale) mod 2^log_size.  extended_omega32 is only read when the program
- * uses B200ZK_SRC_EXTENDED_X (may be NULL otherwise). */
+ * column reads at (row + rotations[r] * rot_scale) mod 2^log_size.  The extended domain is log_size = extended_k with
+ * rot_scale = 2^(extended_k - k) (evaluate_h); log_size = k with rot_scale = 1 is the Lagrange domain, upstream's
+ * `evaluate(expression, n, 1, ...)` (mv-lookup compression of the input / table tuples with theta).  extended_omega32 is only
+ * read when the program uses B200ZK_SRC_EXTENDED_X (may be NULL otherwise). */
 B200ZK_API int32_t b200zk_graph_evaluate(b200zk_ctx* ctx, const b200zk_graph* graph, const void* const* fixed_dev,
                                          uint32_t n_fixed, const void* const* advice_dev, uint32_t n_advice,
                                          const void* const* instance_dev, uint32_t n_instance, const void* challenges32,

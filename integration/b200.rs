@@ -112,6 +112,19 @@ pub(crate) fn graph_evaluate_part(graph: *const sys::Graph, fixed_dev: &[*const 
     });
 }
 
+/// mv_lookup::Argument::prepare's compress_expressions: out_dev[r] = fold(acc * theta + e(r)) over the tuple whose program
+/// (Horner(0, [e_0 .. e_{m-1}], Theta), built once per proving key) is `graph`, on the Lagrange columns of 2^k rows; rotations
+/// wrap mod 2^k.  Every table entry up to the largest index the program reads must be a device column.
+pub(crate) fn compress_expressions(graph: *const sys::Graph, fixed_dev: &[*const c_void], advice_dev: &[*const c_void],
+                                   instance_dev: &[*const c_void], challenges: &[Fr], theta: Fr, out_dev: *mut c_void, k: u32) {
+    let zero = Fr::zero();
+    check(unsafe {
+        sys::b200zk_graph_evaluate(ctx(), graph, fixed_dev.as_ptr(), fixed_dev.len() as u32, advice_dev.as_ptr(), advice_dev.len() as u32,
+                                   instance_dev.as_ptr(), instance_dev.len() as u32, challenges.as_ptr() as _, challenges.len() as u32,
+                                   p(&zero), p(&zero), p(&theta), p(&zero), std::ptr::null(), out_dev, k, 1)
+    });
+}
+
 /// mv_lookup::Argument::prepare, the multiplicity column: m_dev[t] = how many (input, row < usable) cells hold the value of
 /// table row t, counted on the first usable row with that value.  All columns are device memory of 2^k elements.  A value in
 /// no usable table row is the error prepare returns for it (ConstraintSystemFailure), not a panic.

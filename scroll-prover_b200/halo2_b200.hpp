@@ -600,6 +600,27 @@ inline uint64_t lookup_multiplicities(const std::vector<const DeviceColumn*>& in
     return first_missing;
 }
 
+// mv_lookup::Argument::prepare's compress_expressions: out[r] = the value of `graph` at row r of the 2^k Lagrange domain, the graph
+// being a compressed tuple's program (Horner(0, [e_0 .. e_{m-1}], Theta)).  b200zk_graph_evaluate with log_size = k and
+// rot_scale = 1: rotations read (r + rotation) mod 2^k.  Every table entry up to the largest index the program reads must be a
+// device column of 2^k elements; the ABI refuses a shorter table.
+inline void compress_expressions(const b200zk_graph* graph, const EvaluationDomain& dom, const std::vector<const DeviceColumn*>& fixed,
+                                 const std::vector<const DeviceColumn*>& advice, const std::vector<const DeviceColumn*>& instance,
+                                 const std::vector<Fr>& challenges, const Fr& theta, DeviceColumn& out) {
+    if (out.len() != dom.n) throw Panic("compress_expressions: out must hold the 2^k rows of the domain");
+    auto table = [](const std::vector<const DeviceColumn*>& v) {
+        std::vector<const void*> t;
+        for (auto* c : v) t.push_back(c->ptr());
+        return t;
+    };
+    auto tf = table(fixed), ta = table(advice), ti = table(instance);
+    const Fr zero = detail::from_dev(detail::DFr::zero());  // beta, gamma, y: not read by a compression program
+    auto& b = Backend::get();
+    b.check(b200zk_graph_evaluate(b.ctx(), graph, tf.data(), (uint32_t)tf.size(), ta.data(), (uint32_t)ta.size(), ti.data(), (uint32_t)ti.size(),
+                                  challenges.data(), (uint32_t)challenges.size(), &zero, &zero, &theta, &zero, nullptr, out.ptr(), dom.k, 1),
+            "compress_expressions");
+}
+
 }  // namespace plonk
 
 }  // namespace halo2_b200

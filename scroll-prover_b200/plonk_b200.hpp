@@ -11,7 +11,7 @@
 //
 // Every field-vector / group operation of the prover goes through the `Ops` interface below -- exactly the operations
 // libb200zk replaces (commit_lagrange, commit, lagrange_to_coeff, coeff_to_extended, extended_to_coeff, GraphEvaluator,
-// permutation product, lookup multiplicities, log-derivative sum, eval_polynomial, kate_division, linear combinations).  `DeviceOps` implements it
+// permutation product, lookup compression and multiplicities, log-derivative sum, eval_polynomial, kate_division, linear combinations).  `DeviceOps` implements it
 // over the C ABI (include/b200zk.h); the tests implement the same interface over the CPU oracle and require IDENTICAL PROOF
 // BYTES from both.  The host keeps what upstream keeps on the host: the transcript, challenge arithmetic, blinding rows,
 // rotation-set bookkeeping.  The verifier is host-only (pairing_bn254.hpp), as in the reference.
@@ -450,6 +450,15 @@ inline ValueSource add_expression(GraphEvaluator& ev, const Expr& e) {
     }
 }
 
+// mv_lookup's compression of a tuple with theta: Horner(0, [e_0 .. e_{m-1}], Theta) = ((0 * theta + e_0) * theta + e_1) ...,
+// the host fold of compress_expressions (prover.rs) and evaluate_h's `evaluate_lc`
+inline ValueSource add_compressed(GraphEvaluator& ev, const std::vector<ExprP>& exprs) {
+    const ValueSource zero = ev.add_constant(f_zero());
+    std::vector<ValueSource> parts;
+    for (auto& e : exprs) parts.push_back(add_expression(ev, *e));
+    return ev.add_horner(zero, parts, ValueSource::Theta());
+}
+
 // ------------------------------------------------------------------------------------------------ ConstraintSystem
 struct Column {
     int kind;  // Expr::Fixed / Advice / Instance
@@ -573,6 +582,39 @@ struct Ops {
         return m;
     }
     static const char* lookup_missing_message() { return "lookup input is not in the table (the witness does not satisfy the lookup)"; }
+    // mv_lookup::Argument::prepare's compress_expressions for every lookup side of a proof: out[s][r] = fold(acc * theta + e(r))
+    // over the tuple sides[s], from the Lagrange values of the domain (rotations wrap mod n) and the challenges by index.
+    // programs[s] is keygen's lowering of sides[s] (compression_program).  The default is the host fold over the expressions.
+    virtual std::vector<Poly> compress_expressions(const std::vector<const std::vector<ExprP>*>& sides, const std::vector<Program>& programs,
+                                                   const std::vector<Poly>& fixed, const std::vector<Poly>& advice,
+                                                   const std::vector<Poly>& instances, const std::vector<Fr>& challenges, const Fr& theta) {
+        (void)programs;
+        size_t n = 0;
+        for (const auto* cols : {&fixed, &advice, &instances})
+            for (auto& c : *cols) n = std::max(n, c.size());
+        auto lagrange_query = [&](uint64_t row) {
+            return [&, row](int kind, uint32_t col, int32_t rot) -> Fr {
+                uint64_t r = (uint64_t)(((int64_t)row + rot) % (int64_t)n + (int64_t)n) % n;
+                if (kind == Expr::Challenge) return challenges[col];
+                if (kind == Expr::Fixed) return fixed[col][r];
+                if (kind == Expr::Advice) return advice[col][r];
+                return instances[col][r];
+            };
+        };
+        auto compress = [&](const std::vector<ExprP>& exprs) {  // fold(acc * theta + expr) over the rows of the domain
+            Poly out(n);
+            for (uint64_t r = 0; r < n; ++r) {
+                Fr acc = f_zero();
+                auto q = lagrange_query(r);
+                for (auto& e : exprs) acc = f_add(f_mul(acc, theta), e->eval_with(q));
+                out[r] = acc;
+            }
+            return out;
+        };
+        std::vector<Poly> out;
+        for (const auto* side : sides) out.push_back(compress(*side));
+        return out;
+    }
 
     // Coset parts of the extended domain: J = 2^(extended_k - k) parts of n rows, part j = extended rows j, j + J, j + 2J, ...
     // The defaults are the whole-coset operations above, so a backend without part kernels computes the same values.
@@ -697,6 +739,59 @@ class DeviceOps : public Ops {
         if (plonk::lookup_multiplicities(di, t, dom_, usable, m) != UINT64_MAX) throw Panic(lookup_missing_message());
         return m.to_host();
     }
+    // Every column some program reads is uploaded once for all sides (the lookups of a circuit share their selector columns).
+    // A table entry no program reads points at one scratch column: the ABI wants a device column in every entry up to the
+    // largest index read.  A table ends at the supplied columns, so a program reading further is refused by the ABI.
+    std::vector<Poly> compress_expressions(const std::vector<const std::vector<ExprP>*>& sides, const std::vector<Program>& programs,
+                                           const std::vector<Poly>& fixed, const std::vector<Poly>& advice, const std::vector<Poly>& instances,
+                                           const std::vector<Fr>& challenges, const Fr& theta) override {
+        if (programs.size() != sides.size()) throw Panic("compress_expressions: one program per lookup side");
+        const std::vector<Poly>* host[3] = {&fixed, &advice, &instances};
+        std::vector<bool> read[3];
+        auto mark = [&](const b200zk_value_source& s) {
+            const int t = s.kind == B200ZK_SRC_FIXED ? 0 : (s.kind == B200ZK_SRC_ADVICE ? 1 : (s.kind == B200ZK_SRC_INSTANCE ? 2 : -1));
+            if (t < 0) return;
+            if (read[t].size() <= s.index) read[t].resize((size_t)s.index + 1, false);
+            read[t][s.index] = true;
+        };
+        for (auto& p : programs) {
+            for (auto& c : p.calcs) { mark(c.a); mark(c.b); }
+            for (auto& s : p.parts) mark(s);
+        }
+        size_t n_read = 0;
+        for (int t = 0; t < 3; ++t) read[t].resize(std::min(read[t].size(), host[t]->size()));
+        for (int t = 0; t < 3; ++t) n_read += (size_t)std::count(read[t].begin(), read[t].end(), true);
+        std::vector<DeviceColumn> keep;  // the uploaded columns, then the scratch column
+        keep.reserve(n_read + 1);
+        std::vector<const DeviceColumn*> tab[3];
+        bool need_scratch = false;
+        for (int t = 0; t < 3; ++t)
+            for (size_t i = 0; i < read[t].size(); ++i) {
+                if (!read[t][i]) { tab[t].push_back(nullptr); need_scratch = true; continue; }
+                const Poly& c = (*host[t])[i];
+                if (c.size() != dom_.n) throw Panic("compress_expressions: a column the programs read does not hold 2^k rows");
+                keep.emplace_back(c);
+                tab[t].push_back(&keep.back());
+            }
+        if (need_scratch) {
+            keep.emplace_back((size_t)dom_.n);
+            for (auto& v : tab)
+                for (auto& e : v) if (!e) e = &keep.back();
+        }
+        auto& be = Backend::get();
+        DeviceColumn out((size_t)dom_.n);
+        std::vector<Poly> res;
+        for (const Program& p : programs) {
+            b200zk_graph* raw = nullptr;
+            be.check(b200zk_graph_create(be.ctx(), p.calcs.data(), (uint32_t)p.calcs.size(), p.parts.data(), (uint32_t)p.parts.size(),
+                                         p.constants.data(), (uint32_t)p.constants.size(), p.rotations.data(), (uint32_t)p.rotations.size(), &raw),
+                     "compress_expressions: graph_create");
+            std::unique_ptr<b200zk_graph, void (*)(b200zk_graph*)> g(raw, [](b200zk_graph* x) { b200zk_graph_destroy(Backend::get().ctx(), x); });
+            plonk::compress_expressions(g.get(), dom_, tab[0], tab[1], tab[2], challenges, theta, out);
+            res.push_back(out.to_host());
+        }
+        return res;
+    }
 
   private:
     // part < 0: the whole extended coset (b200zk_graph_evaluate); else that coset part (b200zk_graph_evaluate_part)
@@ -773,9 +868,17 @@ struct ProvingKey {
     Program gates;                                        // custom gates folded with y
     Program permutation;                                  // evaluate_h "Permutations" section
     std::vector<Program> lookups;                         // one program per lookup
+    std::vector<Program> lookup_compression;              // per lookup: its input tuple's compression, then its table's
 };
 
 inline Program take_program(const GraphEvaluator& ev) { return Program{ev.calculations(), ev.horner_parts(), ev.constants(), ev.rotations()}; }
+
+// the standalone program of one compressed tuple (add_compressed), for Ops::compress_expressions
+inline Program compression_program(const std::vector<ExprP>& exprs) {
+    GraphEvaluator ev;
+    add_compressed(ev, exprs);
+    return take_program(ev);
+}
 
 inline Fr vk_transcript_repr(const VerifyingKey& vk) {
     Blake2b h("Halo2-Verify-Key");
@@ -917,17 +1020,14 @@ inline ProvingKey keygen(Ops& ops, const EvaluationDomain& dom, ConstraintSystem
         GraphEvaluator ev;
         const uint32_t r0 = ev.add_rotation(0);
         const uint32_t base = aux.z0 + aux.n_sets + 2 * (uint32_t)li;
-        const ValueSource zero = ev.add_constant(f_zero());
-        auto compress = [&](const std::vector<ExprP>& exprs) {
-            std::vector<ValueSource> parts;
-            for (auto& e : exprs) parts.push_back(add_expression(ev, *e));
-            return ev.add_horner(zero, parts, ValueSource::Theta());
-        };
-        const ValueSource input = compress(cs.lookups[li].inputs), table = compress(cs.lookups[li].table);
+        const ValueSource input = add_compressed(ev, cs.lookups[li].inputs), table = add_compressed(ev, cs.lookups[li].table);
         lookup_constraints(ev, {input}, table, ValueSource::Advice(base, r0), ValueSource::Advice(base + 1, r0), ValueSource::Fixed(aux.l0, r0),
                            ValueSource::Fixed(aux.l_last, r0), ValueSource::Fixed(aux.l_active, r0));
         pk.lookups.push_back(take_program(ev));
     }
+    // mv_lookup::Argument::prepare: the same compression alone, evaluated on the Lagrange values of the base domain
+    for (auto& l : cs.lookups)
+        for (const auto* side : {&l.inputs, &l.table}) pk.lookup_compression.push_back(compression_program(*side));
     return pk;
 }
 
@@ -1105,30 +1205,17 @@ inline ProofArtifacts create_proof(Ops& ops, const EvaluationDomain& dom, const 
     const Fr theta = tr.squeeze_challenge();
 
     // 2. lookups, first half (mv_lookup::Argument::prepare): compress with theta, count multiplicities, commit m
-    auto lagrange_query = [&](uint64_t row) {
-        return [&, row](int kind, uint32_t col, int32_t rot) -> Fr {
-            uint64_t r = (uint64_t)(((int64_t)row + rot) % (int64_t)n + (int64_t)n) % n;
-            if (kind == Expr::Challenge) return challenges[col];
-            if (kind == Expr::Fixed) return pk.fixed_values[col][r];
-            if (kind == Expr::Advice) return advice[col][r];
-            return instances[col][r];
-        };
-    };
-    auto compress = [&](const std::vector<ExprP>& exprs) {  // fold(acc * theta + expr) over the rows of the domain
-        Poly out(n);
-        for (uint64_t r = 0; r < n; ++r) {
-            Fr acc = f_zero();
-            auto q = lagrange_query(r);
-            for (auto& e : exprs) acc = f_add(f_mul(acc, theta), e->eval_with(q));
-            out[r] = acc;
-        }
-        return out;
-    };
+    std::vector<const std::vector<ExprP>*> sides;  // per lookup: input tuple, then table tuple (pk.lookup_compression's order)
+    for (auto& l : cs.lookups) {
+        sides.push_back(&l.inputs);
+        sides.push_back(&l.table);
+    }
+    std::vector<Poly> compressed = ops.compress_expressions(sides, pk.lookup_compression, pk.fixed_values, advice, instances, challenges, theta);
     struct LookupState { Poly input, table, m, phi, m_poly, phi_poly; };
     std::vector<LookupState> lk(cs.lookups.size());
     for (size_t li = 0; li < cs.lookups.size(); ++li) {
-        lk[li].input = compress(cs.lookups[li].inputs);
-        lk[li].table = compress(cs.lookups[li].table);
+        lk[li].input = std::move(compressed[2 * li]);
+        lk[li].table = std::move(compressed[2 * li + 1]);
         lk[li].m = ops.lookup_multiplicities({&lk[li].input}, lk[li].table, u);
         write_point(ops.commit_lagrange(lk[li].m));
     }
