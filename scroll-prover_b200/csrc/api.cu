@@ -50,7 +50,6 @@ int32_t b200zk_ctx_create(const int* devices, int n_devices, b200zk_ctx** out) {
     ctx->own_stream = true;
     if (const char* e = getenv("B200ZK_OVERLAP")) ctx->overlap = atoi(e);
     if (const char* e = getenv("B200ZK_ACC_L")) ctx->msm_acc_l = (uint32_t)atoi(e);
-    if (const char* e = getenv("B200ZK_SCATTER_SWEEPS")) ctx->msm_scatter_sweeps = (uint32_t)atoi(e);  // experiment knob
     if (cudaMalloc(&ctx->msm_adds_dev, 8) == cudaSuccess) cudaMemset(ctx->msm_adds_dev, 0, 8);
     else ctx->msm_adds_dev = nullptr;
     *out = ctx;

@@ -75,7 +75,6 @@ struct b200zk_ctx {
     uint64_t prof_cnt[b200zk::PROF_NKEYS] = {0};
     // msm knobs / stats
     uint32_t msm_window = 0;
-    uint32_t msm_scatter_sweeps = 0;
     uint32_t msm_acc_l = 0;
     int srs_precompute = 1;  // 1 auto: SRS handles of >= 2^16 points keep 2^(c*w) multiples when memory allows
     unsigned long long* msm_adds_dev = nullptr;  // running count of bucket additions actually performed

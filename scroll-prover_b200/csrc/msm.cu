@@ -7,10 +7,12 @@
 // sum_i s_i * P_i, returned normalised, so its bytes equal the reference's `to_affine()` output.
 //
 // Pipeline (DESIGN.md "MSM"); all of it on the context stream, no host synchronisation inside:
-//   1 msm_count       scalar -> canonical (one Montgomery product), signed c-bit digits -> digits[w*n+i], histogram
-//   2 scan            exclusive prefix sum of the bucket counts (three kernels)
-//   3 msm_scatter     counting sort of (table index | sign) into bucket order; window-major / a few bucket-range
-//                     sweeps so that the random 4-byte stores fall into a narrower region
+//   1 msm_count       scalar -> canonical (one Montgomery product), signed c-bit digits -> digits[w*n+i]; digits per
+//                     coarse bin (256 buckets) counted in shared memory
+//   2 scan            exclusive prefix sum of the bin counts (three kernels)
+//   3 msm_partition + msm_bin_sort (+ msm_big_* for giant bins)   two-level counting sort of (table index | sign) into
+//                     bucket order: tiles ordered by bin in shared memory and written as runs, then every bin ordered by
+//                     its fine key; no global atomic per digit
 //   4 msm_accumulate  lock-step segmented reduction: every thread owns L consecutive sorted entries and adds affine
 //                     bases into an XYZZ accumulator (8M+2S per add); buckets wholly inside a chunk are stored
 //                     directly, the <= 2 cut runs become partial records
@@ -21,7 +23,7 @@
 //   7 msm_finish      one block per column: Horner over the bit sums and the bucket sets, normalisation to (x, y, 1)
 // With a precomputed SRS (tables 2^(c*w) P_i, built at registration) all windows share ONE bucket set.
 // BATCHES: up to 32 columns over the same bases run through one pipeline (bucket set = column * Ws + window; the grids of
-// count / scatter carry the column in blockIdx.y), so the fixed phases are paid once per batch (msm_run_batch).
+// count / partition carry the column in blockIdx.y), so the fixed phases are paid once per batch (msm_run_batch).
 // Zero scalars and zero digits are skipped (witness columns are mostly zeros / small values).
 #include "common.cuh"
 #include "ec.cuh"
@@ -60,30 +62,83 @@ __device__ __forceinline__ void ld_affine(const Affine* p, Fq& x, Fq& y) {
     y.l.v[4] = d.x; y.l.v[5] = d.y; y.l.v[6] = d.z; y.l.v[7] = d.w;
 }
 
-// every scalar once: canonical form, signed digits -> digits[w*n + i] (magnitude | sign<<31, 0 = skip) + histogram
-__global__ void __launch_bounds__(256) msm_count(MsmCols cols, uint64_t n, MsmPlan pl, uint32_t* hist, uint32_t* digits_all) {
-    // grid = (blocks over the scalars, column of the batch): no 64-bit division per element
+// ---- bucket sort: a two-level counting sort with no global atomic per digit ----------------------------------------
+// A bucket b of set s has the global id s*B + b.  Its COARSE BIN is b >> FB: K = B >> FB bins per set of F = 2^FB buckets
+// each (FB = min(8, c - 1), so that the FINE key b & (F - 1) is one byte).  Bin id = s*K + b>>FB, hence bucket id = bin*F +
+// fine, and bins in id order are buckets in id order.
+//   msm_count      recode every scalar once -> digits[w*n + i]; count digits per bin in shared memory, one global add per
+//                  (block, bin)
+//   scan           exclusive prefix sum of the bin counts -> bin_off (and bin_cur, the partition's cursors)
+//   msm_partition  a block takes a tile of one window's digits, counts its bins in shared memory, reserves one contiguous
+//                  run per bin (one global add per (tile, bin)), orders the tile by bin in shared memory and writes entry +
+//                  fine key linearly into the runs.  Concurrent blocks reserve neighbouring runs, so L2 merges the run ends
+//   msm_bin_sort   one block per bin: counting sort by the fine key, SORT_CH entries at a time ordered in shared memory,
+//                  writes the bin's F offsets and its entries in bucket order
+//   msm_big_*      bins above SORT_BIG entries (a giant bucket: millions of equal digits) are split over a whole grid instead
+static constexpr int SORT_T = 512;                              // threads per block of the sort kernels
+static constexpr int PART_T = 512, PART_ITEMS = 16, PART_TILE = PART_T * PART_ITEMS;  // digits per partition block
+static constexpr uint32_t PART_STAGE_K = 8192;                  // up to this many bins a tile is ordered in shared memory
+static constexpr int SORT_CH = 4096;                            // entries msm_bin_sort orders in shared memory at a time
+static constexpr uint32_t SORT_FB_MAX = 8;                      // fine key = one byte
+static constexpr uint32_t SORT_BIG = 1u << 17;                  // larger bins take the multi-block path
+static constexpr uint32_t COUNT_LOCAL_MAX = 28672;              // bins counted in one block's shared memory (112 KiB)
+
+struct SortPlan {
+    uint32_t FB, K;      // fine bits, bins per bucket set
+    uint32_t wpg;        // windows per msm_count group (plain bases; the precomputed SRS has one set and one group)
+};
+
+__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
+
+// shared-memory add with one atomic per warp when every active lane has the same key (a giant bucket of a skewed witness
+// column puts whole warps on one counter); otherwise one atomic per lane (__match_any_sync grouping costs more than the
+// conflicts it saves on spread keys).  Every lane of the warp must call it.  Returns the old value + this lane's rank.
+__device__ __forceinline__ uint32_t agg_add(uint32_t* ctr, uint32_t key, bool active) {
+    const uint32_t act = __ballot_sync(0xffffffffu, active);
+    const uint32_t kmin = __reduce_min_sync(0xffffffffu, active ? key : 0xffffffffu);
+    const uint32_t kmax = __reduce_max_sync(0xffffffffu, active ? key : 0u);
+    if (act && kmin == kmax) {
+        const uint32_t lane = lane_id(), leader = __ffs(act) - 1;
+        uint32_t base = 0;
+        if (lane == leader) base = atomicAdd(&ctr[kmin], (uint32_t)__popc(act));
+        base = __shfl_sync(0xffffffffu, base, leader);
+        return base + __popc(act & ((1u << lane) - 1));
+    }
+    return active ? atomicAdd(&ctr[key], 1u) : 0u;
+}
+
+// grid = (blocks, column, window group).  Every scalar once: canonical form, signed digits -> digits[w*n + i]
+// (magnitude | sign<<31, 0 = skip) for the windows of this group; bin counts in shared memory, flushed with one global
+// add per (block, bin).
+__global__ void __launch_bounds__(SORT_T) msm_count(MsmCols cols, uint64_t n, MsmPlan pl, SortPlan sp, uint32_t* __restrict__ bin_cnt,
+                                                   uint32_t* __restrict__ digits_all) {
+    extern __shared__ uint32_t lc[];
     const uint32_t col = blockIdx.y;
     const Fr* scalars = cols.p[0];
 #pragma unroll
     for (int q = 1; q < MSM_MAX_BATCH; ++q)
         if (q == (int)col) scalars = cols.p[q];  // no dynamic indexing of kernel parameters
+    const uint32_t wlo = blockIdx.z * sp.wpg, whi = min(pl.W, wlo + sp.wpg);
+    const uint32_t nloc = (pl.Ws == 1 ? 1u : whi - wlo) * sp.K;
+    for (uint32_t b = threadIdx.x; b < nloc; b += blockDim.x) lc[b] = 0;
+    __syncthreads();
     uint32_t* digits = digits_all + (uint64_t)col * pl.W * n;
-    uint32_t* hist_c = hist + (uint64_t)col * pl.Ws * pl.B;
-    uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        Fr s = scalars[i];
-        if (s.is_zero()) {
-            for (uint32_t w = 0; w < pl.W; ++w) digits[(uint64_t)w * n + i] = 0;
-            continue;
-        }
-        s = s.from_mont();
-        uint32_t l[8];
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x; i0 < n; i0 += stride) {  // i0 is block-uniform: whole warps iterate
+        const uint64_t i = i0 + threadIdx.x;
+        const bool ok = i < n;
+        uint32_t l[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        if (ok) {
+            Fr s = scalars[i];
+            if (!s.is_zero()) {
+                s = s.from_mont();
 #pragma unroll
-        for (int k = 0; k < 8; ++k) l[k] = s.l.v[k];
+                for (int k = 0; k < 8; ++k) l[k] = s.l.v[k];
+            }
+        }
         const uint32_t c = pl.c, mask = (1u << c) - 1, half = 1u << (c - 1);
         uint32_t carry = 0;
-        for (uint32_t w = 0; w < pl.W; ++w) {
+        for (uint32_t w = 0; w < whi; ++w) {
             uint32_t v = (l[0] & mask) + carry;
 #pragma unroll
             for (int k = 0; k < 7; ++k) l[k] = __funnelshift_r(l[k], l[k + 1], c);
@@ -97,48 +152,292 @@ __global__ void __launch_bounds__(256) msm_count(MsmCols cols, uint64_t n, MsmPl
                 enc = v;
                 carry = 0;
             }
-            digits[(uint64_t)w * n + i] = enc;
-            if (enc) atomicAdd(&hist_c[(pl.Ws == 1 ? 0ull : (uint64_t)w * pl.B) + (enc & 0x7fffffffu) - 1], 1u);
+            if (w < wlo) continue;
+            if (ok) digits[(uint64_t)w * n + i] = enc;
+            const uint32_t bin = ((enc & 0x7fffffffu) - 1) >> sp.FB;
+            agg_add(lc, (pl.Ws == 1 ? 0u : (w - wlo) * sp.K) + bin, enc != 0);
         }
     }
+    __syncthreads();
+    uint32_t* gc = bin_cnt + ((uint64_t)col * pl.Ws + (pl.Ws == 1 ? 0u : wlo)) * sp.K;
+    for (uint32_t b = threadIdx.x; b < nloc; b += blockDim.x)
+        if (lc[b]) atomicAdd(&gc[b], lc[b]);
 }
 
-// counting-sort scatter in WINDOW-MAJOR order: concurrently running blocks work on the same window, so the
-// random 4-byte stores fall into one n*4-byte region (64 MiB at n = 2^24, most of it held by the 50 MB L2 of an H100)
-// With a precomputed SRS (one bucket set) the destination of a digit is spread over the whole n*W*4-byte entry
-// array, so the kernel is run in SWEEPS over bucket ranges [b_lo, b_hi): each sweep re-reads the digits (coalesced)
-// but writes into a quarter-size region.  On an H100 (50 MB L2) the ~200 MB regions are not L2-resident, yet the narrower
-// store footprint still pays: see the sweep rule in msm_run_batch.
-__global__ void __launch_bounds__(256) msm_scatter(const uint32_t* __restrict__ digits, uint64_t n, MsmPlan pl,
-                                                   uint32_t* cursor, uint32_t* entries, const uint32_t* __restrict__ total_entries,
-                                                   uint32_t sweep, uint32_t max_sweeps) {
-    // the number of sweeps actually used follows the real entry count M (known only on the device): sparse
-    // witness columns have few entries and get a single sweep
-    uint32_t eff = 1;
-    if (max_sweeps > 1) {
-        uint64_t bytes = 4ull * (*total_entries);
-        eff = (uint32_t)((bytes + (1ull << 28) - 1) >> 28);  // regions of <= 256 MiB (a shift: this runs once per thread)
-        eff = eff < 1 ? 1 : (eff > max_sweeps ? max_sweeps : eff);
+// block-wide exclusive scan of ctr[0..K) in place (PART_T threads); returns the total
+__device__ __forceinline__ uint32_t part_block_scan(uint32_t* ctr, uint32_t K, uint32_t* wsum) {
+    const uint32_t per = (K + PART_T - 1) / PART_T, lo = threadIdx.x * per, lane = lane_id(), warp = threadIdx.x >> 5;
+    uint32_t s = 0;
+    for (uint32_t k = 0; k < per; ++k)
+        if (lo + k < K) s += ctr[lo + k];
+    uint32_t x = s;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= (uint32_t)o) x += y;
     }
-    if (sweep >= eff) return;
-    // B is a power of two and eff <= 4: the range bounds need no 64-bit division either
-    const uint32_t b_lo = eff == 3 ? (pl.B / 3) * sweep : (pl.B / eff) * sweep;
-    const uint32_t b_hi = (sweep + 1 == eff) ? pl.B : (eff == 3 ? (pl.B / 3) * (sweep + 1) : (pl.B / eff) * (sweep + 1));
-    // grid = (blocks over the scalars, col * W + w): the digits of one (column, window) are a contiguous run, so neither the
-    // window nor the column needs a 64-bit division per digit; blocks are still issued window-major (x fastest)
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        uint32_t v = lane < PART_T / 32 ? wsum[lane] : 0u;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            uint32_t y = __shfl_up_sync(0xffffffffu, v, o);
+            if (lane >= (uint32_t)o) v += y;
+        }
+        if (lane < PART_T / 32) wsum[lane] = v;  // inclusive over warps
+    }
+    __syncthreads();
+    uint32_t run = (warp ? wsum[warp - 1] : 0u) + x - s;
+    const uint32_t total = wsum[PART_T / 32 - 1];
+    for (uint32_t k = 0; k < per; ++k)
+        if (lo + k < K) {
+            const uint32_t v = ctr[lo + k];
+            ctr[lo + k] = run;
+            run += v;
+        }
+    __syncthreads();
+    return total;
+}
+
+// grid = (tiles of PART_TILE digits, col * W + w): stage the tile's entries by bin.  staged[pos] = (i + w*stride) | sign,
+// fine[pos] = bucket & (F - 1), with pos inside the run this block reserved in its bin (one global add per (tile, bin)).
+// With K <= PART_STAGE_K the tile is first ordered by bin in shared memory, so that a warp's stores fall into a few runs
+// instead of 32 scattered sectors; wider windows write each entry straight into its run.
+__global__ void __launch_bounds__(PART_T) msm_partition(const uint32_t* __restrict__ digits, uint64_t n, MsmPlan pl, SortPlan sp,
+                                                       uint32_t* __restrict__ bin_cur, uint32_t* __restrict__ staged,
+                                                       uint8_t* __restrict__ fine) {
+    extern __shared__ uint32_t lc[];
+    __shared__ uint32_t wsum[PART_T / 32];
     const uint32_t cw = blockIdx.y;
     const uint32_t col = cw / pl.W, w = cw - col * pl.W;
     const uint32_t* dg = digits + (uint64_t)cw * n;
-    uint32_t* cur = cursor + ((uint64_t)col * pl.Ws + (pl.Ws == 1 ? 0u : w)) * pl.B;
+    uint32_t* cur = bin_cur + ((uint64_t)col * pl.Ws + (pl.Ws == 1 ? 0u : w)) * sp.K;
     const uint32_t woff = (uint32_t)((uint64_t)w * pl.stride);
-    uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-        uint32_t d = dg[i];
-        if (!d) continue;
-        uint32_t bk = (d & 0x7fffffffu) - 1;
-        if (bk < b_lo || bk >= b_hi) continue;
-        uint32_t pos = atomicAdd(&cur[bk], 1u);
-        entries[pos] = ((uint32_t)i + woff) | (d & 0x80000000u);
+    const uint32_t K = sp.K, fmask = (1u << sp.FB) - 1;
+    for (uint32_t b = threadIdx.x; b < K; b += blockDim.x) lc[b] = 0;
+    const uint64_t i0 = (uint64_t)blockIdx.x * PART_TILE + threadIdx.x;
+    uint32_t d[PART_ITEMS];
+#pragma unroll
+    for (int k = 0; k < PART_ITEMS; ++k) {
+        const uint64_t i = i0 + (uint64_t)k * PART_T;
+        d[k] = i < n ? dg[i] : 0u;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < PART_ITEMS; ++k) agg_add(lc, ((d[k] & 0x7fffffffu) - 1) >> sp.FB, d[k] != 0);
+    __syncthreads();
+    if (K > PART_STAGE_K) {
+        for (uint32_t b = threadIdx.x; b < K; b += blockDim.x)
+            if (lc[b]) lc[b] = atomicAdd(&cur[b], lc[b]);
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < PART_ITEMS; ++k) {
+            const uint32_t bk = (d[k] & 0x7fffffffu) - 1;
+            const uint32_t pos = agg_add(lc, bk >> sp.FB, d[k] != 0);
+            if (d[k]) {
+                staged[pos] = ((uint32_t)(i0 + (uint64_t)k * PART_T) + woff) | (d[k] & 0x80000000u);
+                fine[pos] = (uint8_t)(bk & fmask);
+            }
+        }
+        return;
+    }
+    uint32_t* gd = lc + K;           // global run start - local run start, per bin
+    uint32_t* se = gd + K;           // the tile's entries ordered by bin
+    uint32_t* sk = se + PART_TILE;   // bin << 8 | fine key
+#pragma unroll 4
+    for (uint32_t b = threadIdx.x; b < K; b += blockDim.x) gd[b] = lc[b] ? atomicAdd(&cur[b], lc[b]) : 0u;
+    __syncthreads();
+    const uint32_t total = part_block_scan(lc, K, wsum);
+    for (uint32_t b = threadIdx.x; b < K; b += blockDim.x) gd[b] -= lc[b];
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < PART_ITEMS; ++k) {
+        const uint32_t bk = (d[k] & 0x7fffffffu) - 1;
+        const uint32_t p = agg_add(lc, bk >> sp.FB, d[k] != 0);
+        if (d[k]) {
+            se[p] = ((uint32_t)(i0 + (uint64_t)k * PART_T) + woff) | (d[k] & 0x80000000u);
+            sk[p] = (bk >> sp.FB) << 8 | (bk & fmask);
+        }
+    }
+    __syncthreads();
+    for (uint32_t t = threadIdx.x; t < total; t += blockDim.x) {
+        const uint32_t key = sk[t], dst = gd[key >> 8] + t;
+        staged[dst] = se[t];
+        fine[dst] = (uint8_t)(key & 0xffu);
+    }
+}
+
+// exclusive scan of the F <= 256 counters in ctr[] (in place) by warp 0; returns nothing, the caller syncs
+__device__ __forceinline__ void fine_exclusive_scan(uint32_t* ctr, uint32_t F) {
+    if (threadIdx.x >= 32) return;
+    const uint32_t lane = lane_id(), per = (F + 31) / 32, lo = lane * per;
+    uint32_t v[8], s = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        v[k] = (k < (int)per && lo + k < F) ? ctr[lo + k] : 0u;
+        s += v[k];
+    }
+    uint32_t x = s;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= (uint32_t)o) x += y;
+    }
+    uint32_t run = x - s;
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+        if (k < (int)per && lo + k < F) {
+            ctr[lo + k] = run;
+            run += v[k];
+        }
+}
+
+__device__ __forceinline__ void bin_range(const uint32_t* bin_off, uint64_t nbins, const uint32_t* total, uint64_t sb,
+                                          uint32_t& start, uint32_t& end) {
+    start = bin_off[sb];
+    end = sb + 1 < nbins ? bin_off[sb + 1] : *total;
+}
+
+// one block per bin: counting sort by the fine key, offsets[bin*F + f] and the bin's sorted entries.  A bin above SORT_BIG
+// entries is only listed (big_list[0] = count, then bin ids) for the multi-block kernels.
+__global__ void __launch_bounds__(SORT_T, 3) msm_bin_sort(const uint32_t* __restrict__ bin_off, uint64_t nbins, SortPlan sp,
+                                                      const uint32_t* __restrict__ staged, const uint8_t* __restrict__ fine,
+                                                      uint32_t* __restrict__ offsets, uint32_t* __restrict__ entries,
+                                                      uint32_t* __restrict__ big_list) {
+    __shared__ uint32_t ctr[1u << SORT_FB_MAX], lc[1u << SORT_FB_MAX], cnt[1u << SORT_FB_MAX], gd[1u << SORT_FB_MAX];
+    __shared__ uint32_t se[SORT_CH];
+    __shared__ uint8_t sf[SORT_CH];
+    const uint64_t sb = blockIdx.x;
+    const uint32_t F = 1u << sp.FB;
+    uint32_t start, end;
+    bin_range(bin_off, nbins, offsets + nbins * F, sb, start, end);
+    if (end - start > SORT_BIG) {
+        if (threadIdx.x == 0) big_list[1 + atomicAdd(big_list, 1u)] = (uint32_t)sb;
+        return;
+    }
+    for (uint32_t f = threadIdx.x; f < F; f += blockDim.x) ctr[f] = 0;
+    __syncthreads();
+    for (uint32_t p0 = start; p0 < end; p0 += SORT_CH) {  // SORT_CH / SORT_T independent loads in flight per thread
+        uint32_t fk[SORT_CH / SORT_T];
+#pragma unroll
+        for (int k = 0; k < SORT_CH / SORT_T; ++k) {
+            const uint32_t p = p0 + k * SORT_T + threadIdx.x;
+            fk[k] = p < end ? fine[p] : 0u;
+        }
+#pragma unroll
+        for (int k = 0; k < SORT_CH / SORT_T; ++k) agg_add(ctr, fk[k], p0 + k * SORT_T + threadIdx.x < end);
+    }
+    __syncthreads();
+    fine_exclusive_scan(ctr, F);
+    __syncthreads();
+    for (uint32_t f = threadIdx.x; f < F; f += blockDim.x) {
+        ctr[f] += start;
+        offsets[sb * F + f] = ctr[f];
+    }
+    // SORT_CH entries at a time: order the chunk by fine key in shared memory, then write it out linearly, so that a
+    // warp's stores fall into a few bucket runs
+    for (uint32_t c0 = start; c0 < end; c0 += SORT_CH) {
+        const uint32_t len = end - c0 < (uint32_t)SORT_CH ? end - c0 : (uint32_t)SORT_CH;
+        for (uint32_t f = threadIdx.x; f < F; f += blockDim.x) lc[f] = 0;
+        __syncthreads();
+        uint32_t e[SORT_CH / SORT_T], fk[SORT_CH / SORT_T];
+#pragma unroll
+        for (int k = 0; k < SORT_CH / SORT_T; ++k) {
+            const uint32_t t = k * SORT_T + threadIdx.x;
+            e[k] = t < len ? staged[c0 + t] : 0u;
+            fk[k] = t < len ? fine[c0 + t] : 0u;
+        }
+#pragma unroll
+        for (int k = 0; k < SORT_CH / SORT_T; ++k) agg_add(lc, fk[k], k * SORT_T + threadIdx.x < len);
+        __syncthreads();
+        for (uint32_t f = threadIdx.x; f < F; f += blockDim.x) cnt[f] = lc[f];
+        __syncthreads();
+        fine_exclusive_scan(lc, F);
+        __syncthreads();
+        for (uint32_t f = threadIdx.x; f < F; f += blockDim.x) {
+            gd[f] = ctr[f] - lc[f];
+            ctr[f] += cnt[f];
+        }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < SORT_CH / SORT_T; ++k) {
+            const bool ok = k * SORT_T + threadIdx.x < len;
+            const uint32_t p = agg_add(lc, fk[k], ok);
+            if (ok) {
+                se[p] = e[k];
+                sf[p] = (uint8_t)fk[k];
+            }
+        }
+        __syncthreads();
+        for (uint32_t t = threadIdx.x; t < len; t += blockDim.x) entries[gd[sf[t]] + t] = se[t];
+        __syncthreads();
+    }
+}
+
+// big bins, pass 1: every block of the grid counts its slice of each listed bin; one global add per (block, bucket)
+__global__ void __launch_bounds__(SORT_T) msm_big_count(const uint32_t* __restrict__ bin_off, uint64_t nbins, SortPlan sp,
+                                                       const uint8_t* __restrict__ fine, const uint32_t* __restrict__ offsets,
+                                                       const uint32_t* __restrict__ big_list, uint32_t* __restrict__ big_cnt) {
+    __shared__ uint32_t ctr[1u << SORT_FB_MAX];
+    const uint32_t F = 1u << sp.FB, nbig = big_list[0];
+    for (uint32_t j = 0; j < nbig; ++j) {
+        uint32_t start, end;
+        bin_range(bin_off, nbins, offsets + nbins * F, big_list[1 + j], start, end);
+        const uint32_t lo = start + (uint32_t)((uint64_t)(end - start) * blockIdx.x / gridDim.x);
+        const uint32_t hi = start + (uint32_t)((uint64_t)(end - start) * (blockIdx.x + 1) / gridDim.x);
+        for (uint32_t f = threadIdx.x; f < F; f += blockDim.x) ctr[f] = 0;
+        __syncthreads();
+        for (uint32_t p0 = lo; p0 < hi; p0 += SORT_T) {
+            const uint32_t p = p0 + threadIdx.x;
+            agg_add(ctr, p < hi ? fine[p] : 0u, p < hi);
+        }
+        __syncthreads();
+        for (uint32_t f = threadIdx.x; f < F; f += blockDim.x)
+            if (ctr[f]) atomicAdd(&big_cnt[(uint64_t)j * 2 * F + f], ctr[f]);
+        __syncthreads();
+    }
+}
+
+// big bins, pass 2: bucket bases from the pass-1 totals; each block reserves its run per bucket (one global add per
+// (block, bucket) on the cursor beside the totals) and scatters its slice into it
+__global__ void __launch_bounds__(SORT_T, 1) msm_big_scatter(const uint32_t* __restrict__ bin_off, uint64_t nbins, SortPlan sp,
+                                                         const uint32_t* __restrict__ staged, const uint8_t* __restrict__ fine,
+                                                         uint32_t* __restrict__ offsets, uint32_t* __restrict__ entries,
+                                                         const uint32_t* __restrict__ big_list, uint32_t* __restrict__ big_cnt) {
+    __shared__ uint32_t base[1u << SORT_FB_MAX], ctr[1u << SORT_FB_MAX];
+    const uint32_t F = 1u << sp.FB, nbig = big_list[0];
+    for (uint32_t j = 0; j < nbig; ++j) {
+        const uint32_t sb = big_list[1 + j];
+        uint32_t start, end;
+        bin_range(bin_off, nbins, offsets + nbins * F, sb, start, end);
+        const uint32_t lo = start + (uint32_t)((uint64_t)(end - start) * blockIdx.x / gridDim.x);
+        const uint32_t hi = start + (uint32_t)((uint64_t)(end - start) * (blockIdx.x + 1) / gridDim.x);
+        uint32_t* tot = big_cnt + (uint64_t)j * 2 * F;
+        for (uint32_t f = threadIdx.x; f < F; f += blockDim.x) {
+            base[f] = tot[f];
+            ctr[f] = 0;
+        }
+        __syncthreads();
+        for (uint32_t p0 = lo; p0 < hi; p0 += SORT_T) {
+            const uint32_t p = p0 + threadIdx.x;
+            agg_add(ctr, p < hi ? fine[p] : 0u, p < hi);
+        }
+        fine_exclusive_scan(base, F);
+        __syncthreads();
+        for (uint32_t f = threadIdx.x; f < F; f += blockDim.x) {
+            if (blockIdx.x == 0) offsets[(uint64_t)sb * F + f] = start + base[f];
+            if (ctr[f]) ctr[f] = start + base[f] + atomicAdd(&tot[F + f], ctr[f]);
+        }
+        __syncthreads();
+        for (uint32_t p0 = lo; p0 < hi; p0 += SORT_T) {
+            const uint32_t p = p0 + threadIdx.x;
+            const bool ok = p < hi;
+            const uint32_t e = ok ? staged[p] : 0u;
+            const uint32_t pos = agg_add(ctr, ok ? fine[p] : 0u, ok);
+            if (ok) entries[pos] = e;
+        }
+        __syncthreads();
     }
 }
 
@@ -618,17 +917,29 @@ static int32_t msm_run_batch(b200zk_ctx* ctx, const Affine* bases, const Fr* con
     const uint32_t ACC_L = ctx->msm_acc_l ? ctx->msm_acc_l : (uint32_t)ACC_L_DEFAULT;
     uint64_t nthreads = (max_entries + ACC_L - 1) / ACC_L;
     if (nthreads == 0) nthreads = 1;
-    uint32_t ntiles = (uint32_t)((pl.NB + SCAN_TILE - 1) / SCAN_TILE);
-    // carve the scratch arena
+    SortPlan sp;
+    sp.FB = pl.c - 1 < SORT_FB_MAX ? pl.c - 1 : SORT_FB_MAX;
+    sp.K = pl.B >> sp.FB;
+    sp.wpg = pl.Ws == 1 ? pl.W : (COUNT_LOCAL_MAX / sp.K < 1 ? 1 : (COUNT_LOCAL_MAX / sp.K < pl.W ? COUNT_LOCAL_MAX / sp.K : pl.W));
+    const uint32_t groups = (pl.W + sp.wpg - 1) / sp.wpg;
+    const uint64_t nbins = pl.NB >> sp.FB;
+    const uint32_t F = 1u << sp.FB;
+    const uint64_t max_big = max_entries / SORT_BIG + 1;
+    uint32_t ntiles = (uint32_t)((nbins + SCAN_TILE - 1) / SCAN_TILE);
+    // carve the scratch arena.  Sort scratch beyond O(NB): digits and entries (4 B per slot each) and the one-byte fine keys,
+    // which share the accumulate's partial records (idle until the sort is done; >= 1 B per slot at the default ACC_L)
     size_t off = 0;
     auto carve = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-    size_t o_hist = carve(4 * (pl.NB + 1)), o_offs = carve(4 * (pl.NB + 1)), o_cursor = carve(4 * (pl.NB + 1));
+    size_t o_offs = carve(4 * (pl.NB + 1));
+    size_t o_bcnt = carve(4 * (nbins + 1)), o_boff = carve(4 * (nbins + 1)), o_bcur = carve(4 * (nbins + 1));
+    size_t o_big = carve(4 * (max_big + 1)), o_bigc = carve(4 * 2 * F * max_big);
     size_t o_tiles = carve(4 * (size_t)(ntiles + 1));
     size_t o_flag = carve(256);
     size_t o_entries = carve(4 * (max_entries + 4));
     size_t o_digits = carve(4 * (max_entries + 4));
     size_t o_buckets = carve(sizeof(XYZZ) * pl.NB);
-    size_t o_pid = carve(4 * 2 * nthreads), o_pval = carve(sizeof(XYZZ) * 2 * nthreads);
+    size_t pval_bytes = sizeof(XYZZ) * 2 * nthreads;
+    size_t o_pid = carve(4 * 2 * nthreads), o_pval = carve(pval_bytes > max_entries + 16 ? pval_bytes : max_entries + 16);
     uint64_t nthreads2 = (2 * nthreads + COMBINE_LR - 1) / COMBINE_LR;
     size_t o_pid2 = carve(4 * 2 * nthreads2), o_pval2 = carve(sizeof(XYZZ) * 2 * nthreads2);
     const uint32_t kc = pl.c / 2;                       // columns = 2^kc, rows = B / 2^kc  (c - 1 = kc + kr)
@@ -640,76 +951,76 @@ static int32_t msm_run_batch(b200zk_ctx* ctx, const Affine* bases, const Fr* con
     size_t o_gr = carve(sizeof(XYZZ) * red_len), o_sums = carve(sizeof(XYZZ) * 2 * (q_max + 1) * sets);
     B2_TRY(scratch_reserve(ctx, ctx->msm_work, off));
     char* base = (char*)ctx->msm_work.p;
-    uint32_t* hist = (uint32_t*)(base + o_hist);
     uint32_t* offsets = (uint32_t*)(base + o_offs);
-    uint32_t* cursor = (uint32_t*)(base + o_cursor);
+    uint32_t* bin_cnt = (uint32_t*)(base + o_bcnt);
+    uint32_t* bin_off = (uint32_t*)(base + o_boff);
+    uint32_t* bin_cur = (uint32_t*)(base + o_bcur);
+    uint32_t* big_list = (uint32_t*)(base + o_big);
+    uint32_t* big_cnt = (uint32_t*)(base + o_bigc);
     uint32_t* tiles = (uint32_t*)(base + o_tiles);
     uint32_t* giant_flag = (uint32_t*)(base + o_flag);
-    uint32_t* entries = (uint32_t*)(base + o_entries);
+    uint32_t* staged = (uint32_t*)(base + o_entries);  // partitioned entries; the sorted ones go to the dead digits
     uint32_t* digits = (uint32_t*)(base + o_digits);
+    uint32_t* entries = digits;
     uint32_t* pid2 = (uint32_t*)(base + o_pid2);
     XYZZ* pval2 = (XYZZ*)(base + o_pval2);
     XYZZ* buckets = (XYZZ*)(base + o_buckets);
     uint32_t* pid = (uint32_t*)(base + o_pid);
     XYZZ* pval = (XYZZ*)(base + o_pval);
+    uint8_t* fine = (uint8_t*)(base + o_pval);
     XYZZ* grpR = (XYZZ*)(base + o_gr);
     XYZZ* red_sums = (XYZZ*)(base + o_sums);
 
     cudaStream_t st = ctx->stream;
-    B2_CUDA(ctx, cudaMemsetAsync(hist, 0, 4 * (pl.NB + 1), st));
+    B2_CUDA(ctx, cudaMemsetAsync(bin_cnt, 0, 4 * (nbins + 1), st));
+    B2_CUDA(ctx, cudaMemsetAsync(big_list, 0, o_tiles - o_big, st));  // list count and the big bins' totals / cursors
     B2_CUDA(ctx, cudaMemsetAsync(giant_flag, 0, 4, st));
     B2_CUDA(ctx, cudaMemsetAsync(buckets, 0, sizeof(XYZZ) * pl.NB, st));
-    uint32_t sblocks = (uint32_t)ctx->sm_count * 8;
+    const size_t count_smem = 4ull * (pl.Ws == 1 ? 1u : sp.wpg) * sp.K;
+    const size_t part_smem = sp.K > PART_STAGE_K ? 4ull * sp.K : 4ull * (2 * sp.K + 2 * PART_TILE);
+    if (!(ctx->smem_optin & (1u << 9))) {
+        // the largest request: K = 2^15 bins of a window of 24 bits (msm_count takes one window per group there)
+        const int most = (int)(4 * (1u << (24 - 1 - SORT_FB_MAX)));
+        B2_CUDA(ctx, cudaFuncSetAttribute(msm_count, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+        B2_CUDA(ctx, cudaFuncSetAttribute(msm_partition, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+        ctx->smem_optin |= 1u << 9;
+    }
     if (n) {
-        uint64_t want = (n + 255) / 256;
-        uint32_t per_col = (sblocks + batch - 1) / batch;
-        uint32_t blocks = (uint32_t)(want < per_col ? want : per_col);
+        // one wave of resident blocks (as many per SM as the bin counters allow); each flushes its counters once
+        int per_sm = 1;
+        B2_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, msm_count, SORT_T, count_smem));
+        if (per_sm < 1) per_sm = 1;
+        uint64_t want = (n + SORT_T - 1) / SORT_T;
+        uint32_t per = ((uint32_t)ctx->sm_count * (uint32_t)per_sm + batch * groups - 1) / (batch * groups);
+        uint32_t blocks = (uint32_t)(want < per ? want : per);
         {
             ProfScope ps_(ctx, PROF_MSM_COUNT);
-            msm_count<<<dim3(blocks, batch), 256, 0, st>>>(colp, n, pl, hist, digits);
+            msm_count<<<dim3(blocks, batch, groups), SORT_T, count_smem, st>>>(colp, n, pl, sp, bin_cnt, digits);
         }
         B2_LAUNCH_CHECK(ctx);
     }
     {
         ProfScope ps_(ctx, PROF_MSM_SCAN);
-        scan_tile_sums<<<ntiles, SCAN_TPB, 0, st>>>(hist, pl.NB, tiles);
+        scan_tile_sums<<<ntiles, SCAN_TPB, 0, st>>>(bin_cnt, nbins, tiles);
         B2_LAUNCH_CHECK(ctx);
         scan_tile_offsets<<<1, SCAN_TPB, 0, st>>>(tiles, ntiles, offsets + pl.NB, ctx->msm_adds_dev);
         B2_LAUNCH_CHECK(ctx);
-        scan_apply<<<ntiles, SCAN_TPB, 0, st>>>(hist, pl.NB, tiles, offsets, cursor);
+        scan_apply<<<ntiles, SCAN_TPB, 0, st>>>(bin_cnt, nbins, tiles, bin_off, bin_cur);
         B2_LAUNCH_CHECK(ctx);
     }
     if (n) {
         {
             ProfScope ps_(ctx, PROF_MSM_SCATTER);
-            uint64_t want = (n + 1023) / 1024;  // 4 digits per thread; grid.y = col * W + w, issued window-major (x fastest)
-            uint32_t blocks = (uint32_t)(want < 0x7fffffffull ? (want ? want : 1) : 0x7fffffffull);
-            {
-                uint32_t sweeps = 1;
-                if (pl.Ws == 1 && batch == 1) {
-                    // each sweep re-reads the digits, so only a few sweeps of ~200 MB pay off.  Measured on an H100 at
-                    // 400 W (tools/scatter_sweeps.py, precomputed SRS, uniform scalars; 1 / 2 / 3 / 4 sweeps): 2^24
-                    // scatter 15.2 / 13.8 / 13.1 / 13.1 ms, 2^25 30.6 / 28.1 / 26.6 / 25.4 ms, 2^22 flat at 3.0 ms.
-                    // The kernel's range split supports at most 4.  B200ZK_SCATTER_SWEEPS overrides the count.
-                    uint64_t region = 200ull << 20;
-                    sweeps = (uint32_t)((4 * max_entries + region - 1) / region);
-                    if (sweeps < 1) sweeps = 1;
-                    if (sweeps > 4) sweeps = 4;
-                    if (ctx->msm_scatter_sweeps) sweeps = ctx->msm_scatter_sweeps;
-                }
-                for (uint32_t sw = 0; sw < sweeps; ++sw) {
-                    // sweeps after the first may turn out to be unnecessary (the real entry count is only known on the device:
-                    // a witness-like column needs one): they get a grid-stride launch of a few blocks per SM, so that an
-                    // early exit costs microseconds instead of the ~0.1 ms that ~200 K empty blocks take to retire
-                    uint32_t bx = blocks;
-                    if (sw > 0) {
-                        uint32_t lean = (uint32_t)ctx->sm_count * 32u / (batch * pl.W) + 1;
-                        if (lean < bx) bx = lean;
-                    }
-                    msm_scatter<<<dim3(bx, batch * pl.W), 256, 0, st>>>(digits, n, pl, cursor, entries, offsets + pl.NB, sw, sweeps);
-                    if (sw + 1 < sweeps) B2_LAUNCH_CHECK(ctx);
-                }
-            }
+            // grid.y = col * W + w, issued window-major (x fastest): concurrent blocks reserve neighbouring runs of one window
+            uint32_t pblocks = (uint32_t)((n + PART_TILE - 1) / PART_TILE);
+            msm_partition<<<dim3(pblocks, batch * pl.W), PART_T, part_smem, st>>>(digits, n, pl, sp, bin_cur, staged, fine);
+            B2_LAUNCH_CHECK(ctx);
+            msm_bin_sort<<<(uint32_t)nbins, SORT_T, 0, st>>>(bin_off, nbins, sp, staged, fine, offsets, entries, big_list);
+            B2_LAUNCH_CHECK(ctx);
+            uint32_t gblocks = (uint32_t)ctx->sm_count * 2;
+            msm_big_count<<<gblocks, SORT_T, 0, st>>>(bin_off, nbins, sp, fine, offsets, big_list, big_cnt);
+            B2_LAUNCH_CHECK(ctx);
+            msm_big_scatter<<<gblocks, SORT_T, 0, st>>>(bin_off, nbins, sp, staged, fine, offsets, entries, big_list, big_cnt);
         }
         B2_LAUNCH_CHECK(ctx);
         uint32_t ablocks = (uint32_t)((nthreads + 255) / 256);
