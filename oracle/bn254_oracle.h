@@ -144,6 +144,14 @@ void oracle_fill_fr(fr_t *out, uint64_t n, uint64_t seed, int witness_like);
 void oracle_fill_points(g1_affine_t *out, uint64_t n, uint64_t seed, int threads);
 void oracle_fill_points_chain(g1_affine_t *out, uint64_t n, uint64_t seed, int threads);
 
+/* ---- test helper, not a restatement of the reference (dft_identity.c) ---- */
+/* out = (r^N - 1) * sum_{i<m} a_i c^i / (w^i r - 1), which equals sum_{j<N} y_j r^j for y_j = sum_i a_i c^i w^(ij):
+ * an O(m) check of a whole transform.  Returns 0, -1 if w^N != 1, -2 if r^N == 1. */
+int oracle_dft_eval_rhs(fr_t *out, const fr_t *a, uint64_t m, const fr_t *c, const fr_t *w, const fr_t *r, uint64_t N,
+                        int threads);
+/* halo2_eval_polynomial(y, n, r) split over threads (the left side of the identity at 2^28 elements) */
+void oracle_eval_polynomial_mt(fr_t *out, const fr_t *y, uint64_t n, const fr_t *r, int threads);
+
 #ifdef __cplusplus
 }
 #endif

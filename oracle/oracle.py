@@ -21,8 +21,8 @@ _SO = os.path.join(_HERE, "liboracle.so")
 
 
 def build(force: bool = False) -> str:
-    srcs = ["bn254_field.c", "bn254_curve.c", "halo2_arith.c", "halo2_domain.c", "halo2_quotient.c", "bn254_oracle.h",
-            "fp_template.h"]
+    srcs = ["bn254_field.c", "bn254_curve.c", "halo2_arith.c", "halo2_domain.c", "halo2_quotient.c", "dft_identity.c",
+            "bn254_oracle.h", "fp_template.h"]
     stale = force or not os.path.exists(_SO) or any(
         os.path.getmtime(os.path.join(_HERE, s)) > os.path.getmtime(_SO) for s in srcs
     )
@@ -404,6 +404,29 @@ def fill_points_chain(n: int, seed: int, threads: int = 8) -> np.ndarray:
     out = np.zeros((n, 8), np.uint64)
     lib.oracle_fill_points_chain(_p(out), C.c_uint64(n), C.c_uint64(seed), C.c_int(threads))
     return out
+
+
+# ---- test helper, not a restatement of the reference (dft_identity.c)
+def dft_eval_rhs(a, c, omega, r, N: int, threads: int | None = None) -> np.ndarray:
+    """(r^N - 1) * sum_i a_i c^i / (omega^i r - 1): equals eval_polynomial(y, r) for the transform
+    y_j = sum_i a_i c^i omega^(ij), j < N.  O(len(a)) on all host threads; raises if omega^N != 1 or r^N == 1."""
+    a = np.ascontiguousarray(a, np.uint64).reshape(-1, 4)
+    c, omega, r = (np.ascontiguousarray(x, np.uint64).reshape(4) for x in (c, omega, r))
+    out = np.zeros(4, np.uint64)
+    rc = lib.oracle_dft_eval_rhs(_p(out), _p(a), C.c_uint64(len(a)), _p(c), _p(omega), _p(r), C.c_uint64(N),
+                                 C.c_int(threads or os.cpu_count() or 8))
+    if rc != 0:
+        raise ValueError({-1: "omega^N != 1", -2: "r^N == 1"}[rc])
+    return out
+
+
+def eval_polynomial_mt(poly, point, threads: int | None = None) -> np.ndarray:
+    """eval_polynomial(poly, point) with the Horner loop split over all host threads (same value)."""
+    poly = np.ascontiguousarray(poly, np.uint64).reshape(-1, 4)
+    point = np.ascontiguousarray(point, np.uint64).reshape(4)
+    r = np.zeros(4, np.uint64)
+    lib.oracle_eval_polynomial_mt(_p(r), _p(poly), C.c_uint64(len(poly)), _p(point), C.c_int(threads or os.cpu_count() or 8))
+    return r
 
 
 # ---- quotient construction (halo2_quotient.c) ------------------------------------------------------------------

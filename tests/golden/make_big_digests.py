@@ -1,6 +1,7 @@
 """Writes tests/golden/big_digests.json: SHA-256 digests of the ORACLE's outputs at BASELINE sizes (MSM 2^22 / 2^24 uniform and
-witness-like, iNTT 2^24, coset NTT 2^26, g_to_lagrange 2^14 / 2^16) on fixed seeded inputs.  tests/test_gpu_exact_big.py holds the
-CUDA path to the live oracle AND to these committed digests, so later rounds cannot drift.  CPU only; takes a few minutes.
+witness-like, iNTT 2^24 and 2^25, coset NTT 2^26, g_to_lagrange 2^14 / 2^16) on fixed seeded inputs.  tests/test_gpu_exact_big.py
+and tests/test_gpu_chunk_shapes.py (iNTT 2^25) hold the CUDA path to the live oracle AND to these committed digests, so later
+rounds cannot drift.  CPU only; takes a few minutes.
 
     python tests/golden/make_big_digests.py
 """
@@ -47,6 +48,8 @@ def main():
     coeff = dom.lagrange_to_coeff(a, threads)
     out["lagrange_to_coeff_24"] = sha(coeff)
     out["coeff_to_extended_26"] = sha(dom.coeff_to_extended(coeff, threads))
+    k = 25
+    out["lagrange_to_coeff_25"] = sha(O.EvaluationDomain(5, k).lagrange_to_coeff(ntt_inputs(k), threads))
     print("ntt done", flush=True)
     for kk in (14, 16):
         g = O.fill_points_chain(1 << kk, 9300 + kk, GEN_THREADS)
