@@ -264,6 +264,23 @@ B200ZK_API int32_t b200zk_lookup_multiplicities(b200zk_ctx* ctx, const void* con
                                                 const void* table_dev, uint32_t k, uint64_t usable, void* m_out_dev,
                                                 uint64_t* first_missing);
 
+/* dev::MockProver::verify_par's checks, each a list of failing flat indices in ascending order: *count_out (host) = how many
+ * fail, rows_out[0 .. min(cap, count)) = the first of them.  rows_out may be host or device memory and may be NULL when
+ * cap = 0 (count only); columns are device memory of 2^k (n) elements.  Any argument outside the stated ranges, or a host
+ * column, is B200ZK_E_INVALID. */
+/* Rows of values_dev (n field elements) that are not zero: a gate's values over the domain. */
+B200ZK_API int32_t b200zk_nonzero_rows(b200zk_ctx* ctx, const void* values_dev, uint64_t n, uint64_t* rows_out, uint64_t cap,
+                                       uint64_t* count_out);
+/* Every (input j, row i < usable) whose value is in no usable table row, as j * 2^k + i (the compressed input and table tuples
+ * of one lookup).  1 <= n_inputs <= 64, k <= 28, usable <= 2^k. */
+B200ZK_API int32_t b200zk_lookup_missing_rows(b200zk_ctx* ctx, const void* const* inputs_dev, uint32_t n_inputs, const void* table_dev,
+                                              uint32_t k, uint64_t usable, uint64_t* rows_out, uint64_t cap, uint64_t* count_out);
+/* Every cell c * 2^k + r of the n_cols columns whose value differs from that of cell next_dev[c * 2^k + r] (device, n_cols * 2^k
+ * entries: the successor of each cell in its copy cycle, permutation::keygen::Assembly's mapping).  n_cols >= 1, k <= 28; a
+ * next entry >= n_cols * 2^k is B200ZK_E_INVALID (count_out and rows_out are then unspecified). */
+B200ZK_API int32_t b200zk_copy_check(b200zk_ctx* ctx, const void* const* cols_dev, uint32_t n_cols, const uint64_t* next_dev, uint32_t k,
+                                     uint64_t* rows_out, uint64_t cap, uint64_t* count_out);
+
 /* plonk::evaluation::GraphEvaluator on the device.  A program is the upstream `calculations` list: calculation i
  * writes intermediate i; operands are ValueSources.  Calculation::Horner(start, parts, factor) names its parts as a
  * range of `horner_parts`.  B200ZK_SRC_EXTENDED_X is an addition over upstream: the point zeta * extended_omega^row of

@@ -140,6 +140,38 @@ pub(crate) fn lookup_multiplicities(inputs_dev: &[*const c_void], table_dev: *co
     Ok(())
 }
 
+/// The failing flat indices of one MockProver check, ascending and all of them: a counting call, then a call sized from the count.
+fn failing_rows(call: impl Fn(*mut u64, u64, *mut u64) -> i32) -> Vec<u64> {
+    let mut count = 0u64;
+    check(call(std::ptr::null_mut(), 0, &mut count));
+    let mut rows = vec![0u64; count as usize];
+    if count > 0 {
+        check(call(rows.as_mut_ptr(), count, &mut count));
+    }
+    rows
+}
+
+/// dev::MockProver::verify_par, gates: the rows where a gate's values (device, n elements) are not zero.
+pub(crate) fn nonzero_rows(values_dev: *const c_void, n: u64) -> Vec<u64> {
+    failing_rows(|rows, cap, count| unsafe { sys::b200zk_nonzero_rows(ctx(), values_dev, n, rows, cap, count) })
+}
+
+/// dev::MockProver::verify_par, lookups: j * 2^k + i of every (compressed input j, row i < usable) in no usable row of the
+/// compressed table.
+pub(crate) fn lookup_missing_rows(inputs_dev: &[*const c_void], table_dev: *const c_void, k: u32, usable: u64) -> Vec<u64> {
+    failing_rows(|rows, cap, count| unsafe {
+        sys::b200zk_lookup_missing_rows(ctx(), inputs_dev.as_ptr(), inputs_dev.len() as u32, table_dev, k, usable, rows, cap, count)
+    })
+}
+
+/// dev::MockProver::verify_par, copy constraints: c * 2^k + r of every cell whose value differs from that of its successor
+/// next_dev[c * 2^k + r] (the permutation Assembly's mapping, flattened; device memory).
+pub(crate) fn copy_check(cols_dev: &[*const c_void], next_dev: *const u64, k: u32) -> Vec<u64> {
+    failing_rows(|rows, cap, count| unsafe {
+        sys::b200zk_copy_check(ctx(), cols_dev.as_ptr(), cols_dev.len() as u32, next_dev, k, rows, cap, count)
+    })
+}
+
 pub(crate) fn eval_polynomial(poly: &[Fr], point: Fr) -> Fr {
     let mut out = Fr::zero();
     check(unsafe { sys::b200zk_eval_poly(ctx(), poly.as_ptr() as _, poly.len() as u64, p(&point), &mut out as *mut Fr as _) });

@@ -101,6 +101,9 @@ def _signatures():
         "b200zk_permutation_product": [vp, C.POINTER(vp), C.POINTER(vp), u32, vp, vp, vp, vp, vp, u32, vp, vp],
         "b200zk_logup_running_sum": [vp, C.POINTER(vp), u32, vp, vp, vp, u32, vp, vp],
         "b200zk_lookup_multiplicities": [vp, C.POINTER(vp), u32, vp, u32, u64, vp, C.POINTER(u64)],
+        "b200zk_nonzero_rows": [vp, vp, u64, vp, u64, C.POINTER(u64)],
+        "b200zk_lookup_missing_rows": [vp, C.POINTER(vp), u32, vp, u32, u64, vp, u64, C.POINTER(u64)],
+        "b200zk_copy_check": [vp, C.POINTER(vp), u32, vp, u32, vp, u64, C.POINTER(u64)],
         "b200zk_graph_create": [vp, vp, u32, vp, u32, vp, u32, vp, u32, C.POINTER(vp)],
         "b200zk_graph_check": [vp, u32, vp, u32, u32, u32, C.POINTER(u32), C.POINTER(u32), C.c_char_p, u64],
         "b200zk_graph_destroy": [vp, vp],
@@ -436,6 +439,42 @@ class Context:
         missing = C.c_uint64()
         self._ck(lib().b200zk_lookup_multiplicities(self._h, ti, len(inputs), pt, k, usable, po, C.byref(missing)))
         return None if missing.value == (1 << 64) - 1 else missing.value
+
+    # ---- dev::MockProver::verify_par's checks: (count, rows) = how many flat indices fail, and the first min(cap, count) of them,
+    # ascending.  cap=None lists all of them (a counting call first).  out: a device tensor of >= cap int64 entries to write
+    # the list into (rows is then its prefix); by default the list comes back as a numpy uint64 array.
+    def _failing_rows(self, call, cap, out):
+        if cap is None:
+            if out is not None:
+                cap = len(out)
+            else:
+                count = C.c_uint64()
+                self._ck(call(None, 0, C.byref(count)))
+                cap = count.value
+        rows = np.zeros(cap, np.uint64) if out is None else out
+        pr, kr = _ptr(rows)
+        count = C.c_uint64()
+        self._ck(call(pr if cap else None, cap, C.byref(count)))
+        return count.value, rows[: min(cap, count.value)]
+
+    def nonzero_rows(self, values, cap: int | None = None, out=None):
+        """Rows of `values` (device, n field elements) that are not zero: a gate's failing rows."""
+        pv, kv = _ptr(values)
+        n = _count(values, 32)
+        return self._failing_rows(lambda r, c, cnt: lib().b200zk_nonzero_rows(self._h, pv, n, r, c, cnt), cap, out)
+
+    def lookup_missing_rows(self, inputs, table, k: int, usable: int, cap: int | None = None, out=None):
+        """Every (input j, row i < usable) whose value is in no usable table row, as j * 2^k + i (device columns of 2^k)."""
+        ti, ki = self._dev_table(inputs)
+        pt, kt = _ptr(table)
+        return self._failing_rows(lambda r, c, cnt: lib().b200zk_lookup_missing_rows(self._h, ti, len(inputs), pt, k, usable, r, c, cnt),
+                                  cap, out)
+
+    def copy_check(self, cols, nxt, k: int, cap: int | None = None, out=None):
+        """Every cell c * 2^k + r whose value differs from that of cell nxt[c * 2^k + r] (device columns, nxt device uint64)."""
+        tc, kc = self._dev_table(cols)
+        pn, kn = _ptr(nxt)
+        return self._failing_rows(lambda r, c, cnt: lib().b200zk_copy_check(self._h, tc, len(cols), pn, k, r, c, cnt), cap, out)
 
     def graph(self, calcs, constants, rotations) -> "Graph":
         return Graph(self, calcs, constants, rotations)

@@ -15,8 +15,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libb200zk.so")
-SOURCES = ["api.cu", "ntt.cu", "msm.cu", "poly.cu", "g1fft.cu", "quotient.cu", "lookup.cu", "comm.cu"]
-HEADERS = ["ff.cuh", "ec.cuh", "common.cuh", os.path.join("..", "..", "include", "b200zk.h"), "graph.hpp", "graph_exec.cuh"]
+SOURCES = ["api.cu", "ntt.cu", "msm.cu", "poly.cu", "g1fft.cu", "quotient.cu", "lookup.cu", "mock.cu", "comm.cu"]
+HEADERS = ["ff.cuh", "ec.cuh", "common.cuh", os.path.join("..", "..", "include", "b200zk.h"), "graph.hpp", "graph_exec.cuh", "lookup.cuh"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100: the one architecture the library is built for
 FLAGS = GENCODE + [ "-O3", "-std=c++17", "-lineinfo",

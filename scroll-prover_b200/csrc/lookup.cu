@@ -10,35 +10,9 @@
 // the comparisons read the table, which stays in L2 for the hot values.  A slot, once claimed, only ever holds rows of one
 // value (a thread only lowers it with atomicMin after comparing equal), so concurrent inserts of equal values meet in the
 // same slot and the result does not depend on the schedule.
-#include "common.cuh"
+#include "lookup.cuh"
 
 namespace b200zk {
-
-constexpr uint32_t LK_EMPTY = 0xFFFFFFFFu;
-
-struct LkKey {
-    uint4 a, b;
-};
-__device__ __forceinline__ LkKey lk_load(const Fr* p) {
-    const uint4* q = reinterpret_cast<const uint4*>(p);
-    return LkKey{q[0], q[1]};
-}
-__device__ __forceinline__ bool lk_eq(const LkKey& x, const LkKey& y) {
-    return ((x.a.x ^ y.a.x) | (x.a.y ^ y.a.y) | (x.a.z ^ y.a.z) | (x.a.w ^ y.a.w) | (x.b.x ^ y.b.x) | (x.b.y ^ y.b.y) |
-            (x.b.z ^ y.b.z) | (x.b.w ^ y.b.w)) == 0;
-}
-// all four 64-bit limbs mixed into the top `log_slots` bits (multiply-xorshift): the range tables of the chunk circuits are
-// consecutive small integers, whose Montgomery limbs differ in every word, but the hash must not rely on that
-__device__ __forceinline__ uint64_t lk_hash(const LkKey& k, uint32_t log_slots) {
-    uint64_t l0 = ((uint64_t)k.a.y << 32) | k.a.x, l1 = ((uint64_t)k.a.w << 32) | k.a.z;
-    uint64_t l2 = ((uint64_t)k.b.y << 32) | k.b.x, l3 = ((uint64_t)k.b.w << 32) | k.b.z;
-    uint64_t h = l0 * 0x9E3779B97F4A7C15ull;
-    h = (h ^ (h >> 29) ^ l1) * 0xBF58476D1CE4E5B9ull;
-    h = (h ^ (h >> 31) ^ l2) * 0x94D049BB133111EBull;
-    h = (h ^ (h >> 30) ^ l3) * 0x9E3779B97F4A7C15ull;
-    h ^= h >> 32;
-    return (h * 0xD6E8FEB86659FD93ull) >> (64 - log_slots);
-}
 
 __global__ void __launch_bounds__(256) lookup_build_kernel(const Fr* table, uint64_t usable, uint32_t* slots, uint32_t log_slots) {
     const uint64_t mask = (1ull << log_slots) - 1, stride = (uint64_t)gridDim.x * blockDim.x;
@@ -66,25 +40,11 @@ __global__ void __launch_bounds__(256) lookup_probe_kernel(const Fr* const* inpu
                                                            unsigned long long* missing) {
     const uint32_t j = blockIdx.y, lane = threadIdx.x & 31;
     const Fr* in = inputs[j];
-    const uint64_t mask = (1ull << log_slots) - 1, stride = (uint64_t)gridDim.x * blockDim.x;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t base = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); base < usable; base += stride) {
         const uint64_t i = base + lane;
-        uint32_t row = LK_EMPTY;
-        bool miss = false;
-        if (i < usable) {
-            const LkKey key = lk_load(in + i);
-            for (uint64_t h = lk_hash(key, log_slots);; h = (h + 1) & mask) {
-                const uint32_t cur = slots[h];
-                if (cur == LK_EMPTY) {
-                    miss = true;
-                    break;
-                }
-                if (lk_eq(lk_load(table + cur), key)) {
-                    row = cur;
-                    break;
-                }
-            }
-        }
+        const uint32_t row = i < usable ? lk_find(lk_load(in + i), table, slots, log_slots) : LK_EMPTY;
+        const bool miss = i < usable && row == LK_EMPTY;
         // range-check inputs are dominated by a few values: one atomic per distinct row of the warp
         const uint32_t peers = __match_any_sync(0xFFFFFFFFu, row);
         if (row != LK_EMPTY && lane == (uint32_t)(__ffs(peers) - 1)) atomicAdd(counts + row, (unsigned long long)__popc(peers));
@@ -108,18 +68,18 @@ __global__ void __launch_bounds__(256) lookup_finish_kernel(const unsigned long 
     }
 }
 
-static uint32_t lk_blocks(b200zk_ctx* ctx, uint64_t n) {
-    uint64_t want = (n + 255) / 256, cap = (uint64_t)ctx->sm_count * 16;
-    if (want > cap) want = cap;
-    return (uint32_t)(want ? want : 1);
+int32_t lookup_build_launch(b200zk_ctx* ctx, const Fr* table, uint64_t usable, uint32_t* slots, uint32_t log_slots) {
+    if (!usable) return B200ZK_OK;
+    lookup_build_kernel<<<lk_blocks(ctx, usable), 256, 0, ctx->stream>>>(table, usable, slots, log_slots);
+    B2_LAUNCH_CHECK(ctx);
+    return B200ZK_OK;
 }
 
 // scratch in ctx->stage_out: input pointer table | missing | counts (usable u64) | slots (>= 2 usable u32, a power of two)
 int32_t lookup_multiplicities_run(b200zk_ctx* ctx, const void* const* inputs, uint32_t n_inputs, const Fr* table, uint32_t k,
                                   uint64_t usable, Fr* m_out, uint64_t* first_missing) {
     const uint64_t n = 1ull << k;
-    uint32_t log_slots = 6;
-    while ((1ull << log_slots) < 2 * usable) ++log_slots;
+    const uint32_t log_slots = lk_log_slots(usable);
     const size_t o_ptr = 0, o_miss = 8 * 64, o_cnt = o_miss + 8, o_slot = o_cnt + 8 * (size_t)usable;
     const size_t total = o_slot + 4 * ((size_t)1 << log_slots);
     B2_TRY(scratch_reserve(ctx, ctx->stage_out, total));
@@ -134,8 +94,7 @@ int32_t lookup_multiplicities_run(b200zk_ctx* ctx, const void* const* inputs, ui
     {
         ProfScope ps_(ctx, PROF_POLY);
         if (usable) {
-            lookup_build_kernel<<<lk_blocks(ctx, usable), 256, 0, ctx->stream>>>(table, usable, slots, log_slots);
-            B2_LAUNCH_CHECK(ctx);
+            B2_TRY(lookup_build_launch(ctx, table, usable, slots, log_slots));
             uint32_t bx = lk_blocks(ctx, usable * n_inputs) / n_inputs;
             dim3 grid(bx ? bx : 1, n_inputs);
             lookup_probe_kernel<<<grid, 256, 0, ctx->stream>>>((const Fr* const*)(base + o_ptr), k, table, usable, slots, log_slots,

@@ -15,6 +15,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -619,6 +620,51 @@ inline void compress_expressions(const b200zk_graph* graph, const EvaluationDoma
     b.check(b200zk_graph_evaluate(b.ctx(), graph, tf.data(), (uint32_t)tf.size(), ta.data(), (uint32_t)ta.size(), ti.data(), (uint32_t)ti.size(),
                                   challenges.data(), (uint32_t)challenges.size(), &zero, &zero, &theta, &zero, nullptr, out.ptr(), dom.k, 1),
             "compress_expressions");
+}
+
+// dev::MockProver::verify_par's checks: every failing flat index, ascending -- a counting call, then a call sized from the count
+template <class Call>
+inline std::vector<uint64_t> failing_rows(Call&& call, const char* what) {
+    auto& b = Backend::get();
+    uint64_t count = 0;
+    b.check(call(nullptr, 0, &count), what);
+    std::vector<uint64_t> rows(count);
+    if (count) b.check(call(rows.data(), count, &count), what);
+    return rows;
+}
+
+// the rows where `values` (a gate evaluated over the domain) is not zero
+inline std::vector<uint64_t> nonzero_rows(const DeviceColumn& values) {
+    auto& b = Backend::get();
+    return failing_rows([&](uint64_t* rows, uint64_t cap, uint64_t* count) {
+        return b200zk_nonzero_rows(b.ctx(), values.ptr(), values.len(), rows, cap, count);
+    }, "nonzero_rows");
+}
+
+// j * n + i of every (input j, row i < usable) whose value is in no usable row of `table`
+inline std::vector<uint64_t> lookup_missing_rows(const std::vector<const DeviceColumn*>& inputs, const DeviceColumn& table,
+                                                 const EvaluationDomain& dom, uint64_t usable) {
+    std::vector<const void*> ti;
+    for (auto* c : inputs) ti.push_back(c->ptr());
+    auto& b = Backend::get();
+    return failing_rows([&](uint64_t* rows, uint64_t cap, uint64_t* count) {
+        return b200zk_lookup_missing_rows(b.ctx(), ti.data(), (uint32_t)ti.size(), table.ptr(), dom.k, usable, rows, cap, count);
+    }, "lookup_missing_rows");
+}
+
+// c * n + r of every cell whose value differs from that of cell next[c * n + r] (host; uploaded for the call)
+inline std::vector<uint64_t> copy_check(const std::vector<const DeviceColumn*>& cols, const std::vector<uint64_t>& next, const EvaluationDomain& dom) {
+    if (next.size() != cols.size() * dom.n) throw Panic("copy_check: next must hold one entry per cell");
+    std::vector<const void*> tc;
+    for (auto* c : cols) tc.push_back(c->ptr());
+    auto& b = Backend::get();
+    void* next_dev = nullptr;
+    b.check(b200zk_buf_alloc(b.ctx(), 8 * (uint64_t)next.size(), &next_dev), "copy_check: alloc");
+    std::unique_ptr<void, void (*)(void*)> keep(next_dev, [](void* p) { b200zk_buf_free(Backend::get().ctx(), p); });
+    b.check(b200zk_buf_upload(b.ctx(), next_dev, next.data(), 8 * (uint64_t)next.size()), "copy_check: upload");
+    return failing_rows([&](uint64_t* rows, uint64_t cap, uint64_t* count) {
+        return b200zk_copy_check(b.ctx(), tc.data(), (uint32_t)tc.size(), (const uint64_t*)next_dev, dom.k, rows, cap, count);
+    }, "copy_check");
 }
 
 }  // namespace plonk

@@ -539,6 +539,81 @@ struct Program {  // a GraphEvaluator program in the ABI's (= upstream's) form
 };
 using Poly = std::vector<Fr>;
 
+// ------------------------------------------------------------------------------------------------ copy constraints
+struct Assembly {  // permutation::keygen::Assembly: the cell mapping built from copy constraints
+    std::vector<std::vector<std::pair<uint32_t, uint32_t>>> mapping;  // mapping[col][row] = (col', row') next cell of the cycle
+    Assembly(size_t n_cols, size_t n) : mapping(n_cols, std::vector<std::pair<uint32_t, uint32_t>>(n)) {
+        for (size_t c = 0; c < n_cols; ++c)
+            for (size_t r = 0; r < n; ++r) mapping[c][r] = {(uint32_t)c, (uint32_t)r};
+    }
+    // copy(left, right): merges the two cycles (swapping successors joins two disjoint cycles)
+    void copy(uint32_t lc, uint32_t lr, uint32_t rc, uint32_t rr) {
+        // walk left's cycle: if right is already in it, nothing to do
+        auto cur = mapping[lc][lr];
+        while (!(cur.first == lc && cur.second == lr)) {
+            if (cur.first == rc && cur.second == rr) return;
+            cur = mapping[cur.first][cur.second];
+        }
+        if (lc == rc && lr == rr) return;
+        std::swap(mapping[lc][lr], mapping[rc][rr]);
+    }
+};
+
+// ------------------------------------------------------------------------------------------------ MockProver's check
+// dev::MockProver::verify_par (src/dev.rs), given the synthesised witness (mock_prove below): every constraint evaluated with plain
+// field arithmetic -- no polynomial, no commitment --
+//   gates on EVERY row of the domain (what the quotient identity demands; a selector that is live on a row whose rotations reach
+//   into the blinding rows shows up here), lookup inputs against the table on the usable rows, copy constraints cell by cell.
+// The failures come gate-major, then lookup-major, then column-major (index in cs.permutation), rows ascending within each.
+struct MockFailure {
+    enum Kind { Gate, Lookup, Permutation } kind;
+    size_t index;  // gate index, lookup index, or index of the column in cs.permutation
+    uint64_t row;
+    bool operator==(const MockFailure& o) const { return kind == o.kind && index == o.index && row == o.row; }
+};
+inline std::vector<MockFailure> mock_check(const ConstraintSystem& cs, const std::vector<Poly>& fixed, const std::vector<Poly>& advice,
+                                           const std::vector<Poly>& instances, const std::vector<Fr>& challenges, const Fr& theta,
+                                           const Assembly& assembly) {
+    size_t n = 0;
+    for (const auto* cols : {&fixed, &advice, &instances})
+        for (auto& c : *cols) n = std::max(n, c.size());
+    const uint64_t u = n - cs.blinding_factors() - 1;
+    auto cell = [&](uint64_t row) {
+        return [&, row](int kind, uint32_t col, int32_t rot) -> Fr {
+            if (kind == Expr::Challenge) return challenges[col];
+            const uint64_t r = (uint64_t)((((int64_t)row + rot) % (int64_t)n + (int64_t)n) % (int64_t)n);
+            return kind == Expr::Fixed ? fixed[col][r] : (kind == Expr::Advice ? advice[col][r] : instances[col][r]);
+        };
+    };
+    std::vector<MockFailure> failures;
+    for (size_t g = 0; g < cs.gates.size(); ++g)
+        for (uint64_t r = 0; r < n; ++r)
+            if (!f_is_zero(cs.gates[g]->eval_with(cell(r)))) failures.push_back({MockFailure::Gate, g, r});
+    for (size_t li = 0; li < cs.lookups.size(); ++li) {
+        auto compress = [&](const std::vector<ExprP>& es, uint64_t r) {
+            Fr acc = f_zero();
+            auto q = cell(r);
+            for (auto& e : es) acc = f_add(f_mul(acc, theta), e->eval_with(q));
+            return std::array<uint64_t, 4>{acc.l[0], acc.l[1], acc.l[2], acc.l[3]};
+        };
+        std::set<std::array<uint64_t, 4>> table;
+        for (uint64_t r = 0; r < u; ++r) table.insert(compress(cs.lookups[li].table, r));
+        for (uint64_t r = 0; r < u; ++r)
+            if (!table.count(compress(cs.lookups[li].inputs, r))) failures.push_back({MockFailure::Lookup, li, r});
+    }
+    auto value = [&](size_t pcol, uint64_t r) {
+        const Column& c = cs.permutation[pcol];
+        return c.kind == Expr::Fixed ? fixed[c.index][r] : (c.kind == Expr::Advice ? advice[c.index][r] : instances[c.index][r]);
+    };
+    for (size_t c = 0; c < cs.permutation.size(); ++c)
+        for (uint64_t r = 0; r < n; ++r) {
+            const auto next = assembly.mapping[c][r];
+            if (!(value(c, r) == value(next.first, next.second))) failures.push_back({MockFailure::Permutation, c, r});
+        }
+    return failures;
+}
+
+// ------------------------------------------------------------------------------------------------ the operations a backend provides
 struct Ops {
     virtual ~Ops() = default;
     virtual G1 commit_lagrange(const Poly& values) = 0;                      // Params::commit_lagrange
@@ -615,6 +690,13 @@ struct Ops {
         for (const auto* side : sides) out.push_back(compress(*side));
         return out;
     }
+    // dev::MockProver::verify_par's check of a synthesised witness (mock_prove): the failures in mock_check's order.  The default
+    // is mock_check itself.
+    virtual std::vector<MockFailure> check_constraints(const ConstraintSystem& cs, const std::vector<Poly>& fixed, const std::vector<Poly>& advice,
+                                                       const std::vector<Poly>& instances, const std::vector<Fr>& challenges, const Fr& theta,
+                                                       const Assembly& assembly) {
+        return mock_check(cs, fixed, advice, instances, challenges, theta, assembly);
+    }
 
     // Coset parts of the extended domain: J = 2^(extended_k - k) parts of n rows, part j = extended rows j, j + J, j + 2J, ...
     // The defaults are the whole-coset operations above, so a backend without part kernels computes the same values.
@@ -660,6 +742,8 @@ struct Ops {
         throw Panic("graph_evaluate_part: this backend evaluates whole cosets only");
     }
 };
+
+inline Program compression_program(const std::vector<ExprP>& exprs);  // keys, below
 
 // The product: every operation through the C ABI.  Host vectors in and out (the ABI stages them); the quotient-construction
 // group takes device-resident columns, which DeviceColumn provides.
@@ -740,60 +824,121 @@ class DeviceOps : public Ops {
         return m.to_host();
     }
     // Every column some program reads is uploaded once for all sides (the lookups of a circuit share their selector columns).
-    // A table entry no program reads points at one scratch column: the ABI wants a device column in every entry up to the
-    // largest index read.  A table ends at the supplied columns, so a program reading further is refused by the ABI.
     std::vector<Poly> compress_expressions(const std::vector<const std::vector<ExprP>*>& sides, const std::vector<Program>& programs,
                                            const std::vector<Poly>& fixed, const std::vector<Poly>& advice, const std::vector<Poly>& instances,
                                            const std::vector<Fr>& challenges, const Fr& theta) override {
         if (programs.size() != sides.size()) throw Panic("compress_expressions: one program per lookup side");
-        const std::vector<Poly>* host[3] = {&fixed, &advice, &instances};
-        std::vector<bool> read[3];
-        auto mark = [&](const b200zk_value_source& s) {
-            const int t = s.kind == B200ZK_SRC_FIXED ? 0 : (s.kind == B200ZK_SRC_ADVICE ? 1 : (s.kind == B200ZK_SRC_INSTANCE ? 2 : -1));
-            if (t < 0) return;
-            if (read[t].size() <= s.index) read[t].resize((size_t)s.index + 1, false);
-            read[t][s.index] = true;
-        };
-        for (auto& p : programs) {
-            for (auto& c : p.calcs) { mark(c.a); mark(c.b); }
-            for (auto& s : p.parts) mark(s);
-        }
-        size_t n_read = 0;
-        for (int t = 0; t < 3; ++t) read[t].resize(std::min(read[t].size(), host[t]->size()));
-        for (int t = 0; t < 3; ++t) n_read += (size_t)std::count(read[t].begin(), read[t].end(), true);
-        std::vector<DeviceColumn> keep;  // the uploaded columns, then the scratch column
-        keep.reserve(n_read + 1);
-        std::vector<const DeviceColumn*> tab[3];
-        bool need_scratch = false;
-        for (int t = 0; t < 3; ++t)
-            for (size_t i = 0; i < read[t].size(); ++i) {
-                if (!read[t][i]) { tab[t].push_back(nullptr); need_scratch = true; continue; }
-                const Poly& c = (*host[t])[i];
-                if (c.size() != dom_.n) throw Panic("compress_expressions: a column the programs read does not hold 2^k rows");
-                keep.emplace_back(c);
-                tab[t].push_back(&keep.back());
-            }
-        if (need_scratch) {
-            keep.emplace_back((size_t)dom_.n);
-            for (auto& v : tab)
-                for (auto& e : v) if (!e) e = &keep.back();
-        }
-        auto& be = Backend::get();
+        const ColumnTables cols = upload_columns(programs, {}, fixed, advice, instances, "compress_expressions");
         DeviceColumn out((size_t)dom_.n);
         std::vector<Poly> res;
         for (const Program& p : programs) {
-            b200zk_graph* raw = nullptr;
-            be.check(b200zk_graph_create(be.ctx(), p.calcs.data(), (uint32_t)p.calcs.size(), p.parts.data(), (uint32_t)p.parts.size(),
-                                         p.constants.data(), (uint32_t)p.constants.size(), p.rotations.data(), (uint32_t)p.rotations.size(), &raw),
-                     "compress_expressions: graph_create");
-            std::unique_ptr<b200zk_graph, void (*)(b200zk_graph*)> g(raw, [](b200zk_graph* x) { b200zk_graph_destroy(Backend::get().ctx(), x); });
-            plonk::compress_expressions(g.get(), dom_, tab[0], tab[1], tab[2], challenges, theta, out);
+            run_lagrange(p, cols, challenges, theta, out, "compress_expressions");
             res.push_back(out.to_host());
         }
         return res;
     }
+    // Every column a gate, a lookup or the permutation reads is uploaded once.  A gate is the program compression_program({gate}),
+    // whose value is the gate's (Horner(0, [e], theta) = e), run on the 2^k Lagrange rows; a lookup compresses its input and table
+    // tuples the same way and lists the inputs in no usable table row; the copy constraints are one call over the permutation
+    // columns with the Assembly's mapping as flat successors.
+    std::vector<MockFailure> check_constraints(const ConstraintSystem& cs, const std::vector<Poly>& fixed, const std::vector<Poly>& advice,
+                                               const std::vector<Poly>& instances, const std::vector<Fr>& challenges, const Fr& theta,
+                                               const Assembly& assembly) override {
+        const uint64_t n = dom_.n, u = n - cs.blinding_factors() - 1;
+        std::vector<Program> gates, lookups;
+        for (auto& g : cs.gates) gates.push_back(compression_program({g}));
+        for (auto& l : cs.lookups) {
+            lookups.push_back(compression_program(l.inputs));
+            lookups.push_back(compression_program(l.table));
+        }
+        std::vector<Program> all = gates;
+        all.insert(all.end(), lookups.begin(), lookups.end());
+        const ColumnTables cols = upload_columns(all, cs.permutation, fixed, advice, instances, "check_constraints");
+        std::vector<MockFailure> failures;
+        DeviceColumn a((size_t)n), b((size_t)n);
+        for (size_t g = 0; g < gates.size(); ++g) {
+            run_lagrange(gates[g], cols, challenges, theta, a, "check_constraints");
+            for (uint64_t r : plonk::nonzero_rows(a)) failures.push_back({MockFailure::Gate, g, r});
+        }
+        for (size_t li = 0; li < cs.lookups.size(); ++li) {
+            run_lagrange(lookups[2 * li], cols, challenges, theta, a, "check_constraints");
+            run_lagrange(lookups[2 * li + 1], cols, challenges, theta, b, "check_constraints");
+            for (uint64_t r : plonk::lookup_missing_rows({&a}, b, dom_, u)) failures.push_back({MockFailure::Lookup, li, r});
+        }
+        if (!cs.permutation.empty()) {
+            std::vector<const DeviceColumn*> pc;
+            for (const Column& c : cs.permutation) pc.push_back(cols.tab[table_of(c.kind)][c.index]);
+            std::vector<uint64_t> next(cs.permutation.size() * n);
+            for (size_t c = 0; c < cs.permutation.size(); ++c) {
+                if (assembly.mapping.at(c).size() != n) throw Panic("check_constraints: the assembly does not map 2^k rows per column");
+                for (uint64_t r = 0; r < n; ++r) next[c * n + r] = (uint64_t)assembly.mapping[c][r].first * n + assembly.mapping[c][r].second;
+            }
+            for (uint64_t f : plonk::copy_check(pc, next, dom_)) failures.push_back({MockFailure::Permutation, (size_t)(f / n), f % n});
+        }
+        return failures;
+    }
 
   private:
+    // The device tables of fixed, advice and instance columns: an entry that some program or `also` reads is that column uploaded;
+    // any other entry up to the largest index read points at one scratch column, because the ABI wants a device column in every
+    // entry.  A table ends at the supplied columns, so a program reading further is refused by the ABI.
+    struct ColumnTables {
+        std::vector<DeviceColumn> keep;  // the uploaded columns, then the scratch column
+        std::vector<const DeviceColumn*> tab[3];
+    };
+    static int table_of(int expr_kind) { return expr_kind == Expr::Fixed ? 0 : (expr_kind == Expr::Advice ? 1 : 2); }
+    ColumnTables upload_columns(const std::vector<Program>& programs, const std::vector<Column>& also, const std::vector<Poly>& fixed,
+                                const std::vector<Poly>& advice, const std::vector<Poly>& instances, const char* what) {
+        const std::vector<Poly>* host[3] = {&fixed, &advice, &instances};
+        std::vector<bool> read[3];
+        auto mark = [&](int t, uint32_t index) {
+            if (read[t].size() <= index) read[t].resize((size_t)index + 1, false);
+            read[t][index] = true;
+        };
+        auto mark_source = [&](const b200zk_value_source& s) {
+            const int t = s.kind == B200ZK_SRC_FIXED ? 0 : (s.kind == B200ZK_SRC_ADVICE ? 1 : (s.kind == B200ZK_SRC_INSTANCE ? 2 : -1));
+            if (t >= 0) mark(t, s.index);
+        };
+        for (auto& p : programs) {
+            for (auto& c : p.calcs) { mark_source(c.a); mark_source(c.b); }
+            for (auto& s : p.parts) mark_source(s);
+        }
+        for (const Column& c : also) {
+            if (c.index >= host[table_of(c.kind)]->size()) throw Panic(std::string(what) + ": a permutation column is not supplied");
+            mark(table_of(c.kind), c.index);
+        }
+        size_t n_read = 0;
+        for (int t = 0; t < 3; ++t) read[t].resize(std::min(read[t].size(), host[t]->size()));
+        for (int t = 0; t < 3; ++t) n_read += (size_t)std::count(read[t].begin(), read[t].end(), true);
+        ColumnTables out;
+        out.keep.reserve(n_read + 1);
+        bool need_scratch = false;
+        for (int t = 0; t < 3; ++t)
+            for (size_t i = 0; i < read[t].size(); ++i) {
+                if (!read[t][i]) { out.tab[t].push_back(nullptr); need_scratch = true; continue; }
+                const Poly& c = (*host[t])[i];
+                if (c.size() != dom_.n) throw Panic(std::string(what) + ": a column the programs read does not hold 2^k rows");
+                out.keep.emplace_back(c);
+                out.tab[t].push_back(&out.keep.back());
+            }
+        if (need_scratch) {
+            out.keep.emplace_back((size_t)dom_.n);
+            for (auto& v : out.tab)
+                for (auto& e : v) if (!e) e = &out.keep.back();
+        }
+        return out;
+    }
+    // one program on the 2^k Lagrange rows (plonk::compress_expressions: log_size = k, rot_scale = 1) into `out`
+    void run_lagrange(const Program& p, const ColumnTables& cols, const std::vector<Fr>& challenges, const Fr& theta, DeviceColumn& out,
+                      const char* what) {
+        auto& be = Backend::get();
+        b200zk_graph* raw = nullptr;
+        be.check(b200zk_graph_create(be.ctx(), p.calcs.data(), (uint32_t)p.calcs.size(), p.parts.data(), (uint32_t)p.parts.size(),
+                                     p.constants.data(), (uint32_t)p.constants.size(), p.rotations.data(), (uint32_t)p.rotations.size(), &raw),
+                 (std::string(what) + ": graph_create").c_str());
+        std::unique_ptr<b200zk_graph, void (*)(b200zk_graph*)> g(raw, [](b200zk_graph* x) { b200zk_graph_destroy(Backend::get().ctx(), x); });
+        plonk::compress_expressions(g.get(), dom_, cols.tab[0], cols.tab[1], cols.tab[2], challenges, theta, out);
+    }
     // part < 0: the whole extended coset (b200zk_graph_evaluate); else that coset part (b200zk_graph_evaluate_part)
     void run_graph(const Program& p, const std::vector<const Poly*>& fixed, const std::vector<const Poly*>& advice,
                    const std::vector<const Poly*>& instance, const std::vector<Fr>& challenges, const Fr& beta, const Fr& gamma,
@@ -833,25 +978,6 @@ class DeviceOps : public Ops {
 };
 
 // ------------------------------------------------------------------------------------------------ keys
-struct Assembly {  // permutation::keygen::Assembly: the cell mapping built from copy constraints
-    std::vector<std::vector<std::pair<uint32_t, uint32_t>>> mapping;  // mapping[col][row] = (col', row') next cell of the cycle
-    Assembly(size_t n_cols, size_t n) : mapping(n_cols, std::vector<std::pair<uint32_t, uint32_t>>(n)) {
-        for (size_t c = 0; c < n_cols; ++c)
-            for (size_t r = 0; r < n; ++r) mapping[c][r] = {(uint32_t)c, (uint32_t)r};
-    }
-    // copy(left, right): merges the two cycles (swapping successors joins two disjoint cycles)
-    void copy(uint32_t lc, uint32_t lr, uint32_t rc, uint32_t rr) {
-        // walk left's cycle: if right is already in it, nothing to do
-        auto cur = mapping[lc][lr];
-        while (!(cur.first == lc && cur.second == lr)) {
-            if (cur.first == rc && cur.second == rr) return;
-            cur = mapping[cur.first][cur.second];
-        }
-        if (lc == rc && lr == rr) return;
-        std::swap(mapping[lc][lr], mapping[rc][rr]);
-    }
-};
-
 struct VerifyingKey {
     uint32_t k = 0;
     ConstraintSystem cs;
@@ -1487,21 +1613,19 @@ inline ProofArtifacts create_proof(Ops& ops, const EvaluationDomain& dom, const 
     return create_proof(ops, dom, pk, fill, instances, rng_seed, transcript_kind);
 }
 
-// ------------------------------------------------------------------------------------------------ MockProver (host only)
+// ------------------------------------------------------------------------------------------------ MockProver
 // dev::MockProver::run + verify, the check the reference's `make mock` performs before any proving
 // (/root/reference/integration/src/mock.rs:11-30 -> MockProver::verify_par): the witness is synthesised phase by phase (challenges
 // from `seed` instead of a transcript), the rows beyond the usable ones are filled with random values as create_proof would blind
-// them, and every constraint is evaluated with plain field arithmetic -- no polynomial, no commitment, no device:
-//   gates on EVERY row of the domain (what the quotient identity demands; a selector that is live on a row whose rotations reach
-//   into the blinding rows shows up here), lookup inputs against the table on the usable rows, copy constraints cell by cell.
-struct MockFailure {
-    enum Kind { Gate, Lookup, Permutation } kind;
-    size_t index;  // gate index, lookup index, or index of the column in cs.permutation
-    uint64_t row;
-    bool operator==(const MockFailure& o) const { return kind == o.kind && index == o.index && row == o.row; }
+// them, and the constraints are checked by mock_check (host only) or by ops.check_constraints (the same list, from any backend).
+struct MockWitness {
+    ConstraintSystem cs;  // finalized
+    std::vector<Poly> advice;
+    std::vector<Fr> challenges;
+    Fr theta;
 };
-inline std::vector<MockFailure> mock_prove(const EvaluationDomain& dom, ConstraintSystem cs, const std::vector<Poly>& fixed, const Assembly& assembly,
-                                           const WitnessFn& synthesize, const std::vector<Poly>& instances, uint64_t seed = 1) {
+inline MockWitness mock_synthesize(const EvaluationDomain& dom, ConstraintSystem cs, const std::vector<Poly>& fixed, const WitnessFn& synthesize,
+                                   const std::vector<Poly>& instances, uint64_t seed) {
     if (cs.advice_queries.empty() && cs.fixed_queries.empty()) cs.finalize();
     const uint64_t n = dom.n, u = n - cs.blinding_factors() - 1;
     if (fixed.size() != cs.num_fixed || instances.size() != cs.num_instance) throw Panic("mock_prove: wrong number of columns");
@@ -1521,39 +1645,18 @@ inline std::vector<MockFailure> mock_prove(const EvaluationDomain& dom, Constrai
             if (cs.challenge_phase[i] == phase) challenges[i] = rng.fr();
     }
     const Fr theta = rng.fr();
-    auto cell = [&](uint64_t row) {
-        return [&, row](int kind, uint32_t col, int32_t rot) -> Fr {
-            if (kind == Expr::Challenge) return challenges[col];
-            const uint64_t r = (uint64_t)((((int64_t)row + rot) % (int64_t)n + (int64_t)n) % (int64_t)n);
-            return kind == Expr::Fixed ? fixed[col][r] : (kind == Expr::Advice ? advice[col][r] : instances[col][r]);
-        };
-    };
-    std::vector<MockFailure> failures;
-    for (size_t g = 0; g < cs.gates.size(); ++g)
-        for (uint64_t r = 0; r < n; ++r)
-            if (!f_is_zero(cs.gates[g]->eval_with(cell(r)))) failures.push_back({MockFailure::Gate, g, r});
-    for (size_t li = 0; li < cs.lookups.size(); ++li) {
-        auto compress = [&](const std::vector<ExprP>& es, uint64_t r) {
-            Fr acc = f_zero();
-            auto q = cell(r);
-            for (auto& e : es) acc = f_add(f_mul(acc, theta), e->eval_with(q));
-            return std::array<uint64_t, 4>{acc.l[0], acc.l[1], acc.l[2], acc.l[3]};
-        };
-        std::set<std::array<uint64_t, 4>> table;
-        for (uint64_t r = 0; r < u; ++r) table.insert(compress(cs.lookups[li].table, r));
-        for (uint64_t r = 0; r < u; ++r)
-            if (!table.count(compress(cs.lookups[li].inputs, r))) failures.push_back({MockFailure::Lookup, li, r});
-    }
-    auto value = [&](size_t pcol, uint64_t r) {
-        const Column& c = cs.permutation[pcol];
-        return c.kind == Expr::Fixed ? fixed[c.index][r] : (c.kind == Expr::Advice ? advice[c.index][r] : instances[c.index][r]);
-    };
-    for (size_t c = 0; c < cs.permutation.size(); ++c)
-        for (uint64_t r = 0; r < n; ++r) {
-            const auto next = assembly.mapping[c][r];
-            if (!(value(c, r) == value(next.first, next.second))) failures.push_back({MockFailure::Permutation, c, r});
-        }
-    return failures;
+    return MockWitness{std::move(cs), std::move(advice), std::move(challenges), theta};
+}
+inline std::vector<MockFailure> mock_prove(const EvaluationDomain& dom, ConstraintSystem cs, const std::vector<Poly>& fixed, const Assembly& assembly,
+                                           const WitnessFn& synthesize, const std::vector<Poly>& instances, uint64_t seed = 1) {
+    const MockWitness w = mock_synthesize(dom, std::move(cs), fixed, synthesize, instances, seed);
+    return mock_check(w.cs, fixed, w.advice, instances, w.challenges, w.theta, assembly);
+}
+inline std::vector<MockFailure> mock_prove(Ops& ops, const EvaluationDomain& dom, ConstraintSystem cs, const std::vector<Poly>& fixed,
+                                           const Assembly& assembly, const WitnessFn& synthesize, const std::vector<Poly>& instances,
+                                           uint64_t seed = 1) {
+    const MockWitness w = mock_synthesize(dom, std::move(cs), fixed, synthesize, instances, seed);
+    return ops.check_constraints(w.cs, fixed, w.advice, instances, w.challenges, w.theta, assembly);
 }
 
 // ------------------------------------------------------------------------------------------------ snark-verifier protocol export
